@@ -9,6 +9,7 @@ Yee FDTD, Boris pusher, order-3 Esirkepov deposition, fp64).
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for the definition of every field.
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -30,19 +31,30 @@ def emit_line(line):
         sys.stdout.write(data.decode()); sys.stdout.flush()
     else:
         os.write(_LINE_FD, data)
-FALLBACK_HBM_GBS = 6650.0      # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_PEAK_GBS = 3350.0          # H100 SXM data sheet (HBM3, 3.35 TB/s)
+HBM_PEAK_SOURCE = "NVIDIA H100 SXM data sheet (3.35 TB/s)"
 
 
-def measured_peaks():
+def device_info(gpu_index):
+    """Name, power limit and maximum SM clock of the card the numbers are measured on (read-only queries)."""
+    info = {"name": None, "power_limit_w": None, "sm_max_mhz": None}
     try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return json.load(f), "measured (MEASURED_PEAKS.json)"
+        import torch
+        info["name"] = torch.cuda.get_device_name(gpu_index)
     except Exception:
-        return {"hbm_gbs": FALLBACK_HBM_GBS}, "fallback (B200_PROFILING.md)"
+        pass
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        f = [v.strip() for v in out.strip().split(",")]
+        info["power_limit_w"], info["sm_max_mhz"] = float(f[0]), float(f[1])
+    except Exception:
+        pass
+    return info
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """SM clocks / throttle reasons during the timed region (NVML, else an nvidia-smi query loop)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -52,7 +64,7 @@ class ClockSampler:
 
     def start(self):
         # NVML (pynvml) when it loads: a sample every 5 ms, so that even a 100 ms timed region is covered;
-        # otherwise the nvidia-smi loop of the recipe (one sample per 100 ms)
+        # otherwise an nvidia-smi query loop (one sample per 100 ms)
         self.nvml_rows, self._stop, self._thread = [], threading.Event(), None
         try:
             import pynvml
@@ -135,7 +147,7 @@ def cpu_reference_run(n, ppc, steps, warmup, nox=3, use_filter=False, solver="ye
     os.environ.setdefault("OMP_WAIT_POLICY", "active")
     from oracle import oracle
     from warpx_b200 import abi, workloads
-    oracle.build(ref=False)
+    oracle.lib()                 # as build() left it; compiled here only when it is missing
     # same cell size and plasma as the GPU run (dx = 40um/256), smaller box
     lx = 40.0e-6 * n / 256.0
     wl = workloads.uniform_plasma_3d(n=n, ppc=ppc, lx=lx)
@@ -191,6 +203,38 @@ def run_reference(args):
             "cpu_baseline": {k: r[k] for k in ("value", "unit", "cores", "kind", "sample")},
             "e2e": {"value": r["value"], "unit": "particle-steps/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     emit_line(line)
+
+
+DUMP_FIELD_POINTS = 1 << 18        # per component: 9 x 2 MB
+DUMP_PARTICLES = 1 << 18           # 8 arrays x 2 MB
+
+
+def dump_outputs(sim, out_dir, npart_local):
+    """What the timed steps computed, as a caller of Simulation.Evolve receives it: the FieldEnergy diagnostic, the
+    field components Ex..jz at a fixed, seeded sample of their valid points ([k, j, i] order), and the particle
+    arrays (x y z w ux uy uz) of a fixed, seeded sample of particle ids, ordered by id.  The sample depends on the
+    grid and particle count only, so two builds run with the same arguments can be compared array by array."""
+    import numpy as np
+    import torch
+    from warpx_b200 import abi
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "field_energy.npy"), np.array(sim.field_energy(), dtype=np.float64))
+    rng = np.random.default_rng(20240917)
+    for c, name in enumerate(abi.COMP_NAMES):
+        valid = sim.data[c][sim.fab[c].valid_slices()]
+        n = valid.numel()
+        idx = np.sort(rng.choice(n, size=min(n, DUMP_FIELD_POINTS), replace=False))
+        sample = valid.reshape(-1)[torch.from_numpy(idx).to(valid.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), sample.cpu().numpy().astype(np.float64))
+    sp = sim.species[0]
+    want = torch.from_numpy(np.sort(rng.choice(npart_local, size=min(npart_local, DUMP_PARTICLES), replace=False)))
+    ids = sp.id_array()
+    keep = torch.isin(ids, want.to(ids.device))
+    order = torch.argsort(ids[keep])
+    np.save(os.path.join(out_dir, "particle_id.npy"), ids[keep][order].cpu().numpy().astype(np.float64))
+    for name in sp.NAMES:
+        np.save(os.path.join(out_dir, "particle_" + name + ".npy"),
+                sp.array(name)[keep][order].cpu().numpy().astype(np.float64))
 
 
 def start_watchdog(rank):
@@ -304,6 +348,8 @@ def run_engine(args):
     stage = sim.stage_ms()                               # {stage: (ms per call, calls)} of the timed steps
     sim.enable_stage_timing(False)
     fe = sim.field_energy()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(sim, args.dump_outputs, npart_local)
     value = ntot * args.steps / (ms * 1e-3)
     sim.close()
     del sim
@@ -351,8 +397,7 @@ def run_engine(args):
         return
 
     # =================== roofline of the kernels (algorithmic bytes / CUDA-event time) ==========
-    peaks, peak_src = measured_peaks()
-    hbm = float(peaks.get("hbm_gbs", FALLBACK_HBM_GBS))
+    hbm = HBM_PEAK_GBS
     ncell = n ** 3
     alg = {  # bytes per launch, DESIGN.md "Kernels"
         "evolve_b": 72.0 * ncell,
@@ -361,21 +406,15 @@ def run_engine(args):
         "deposit": 56.0 * npart_local + 72.0 * ncell,
         "filter_j": 48.0 * ncell,        # --filter 1: three components, one read + one write each (no copy back)
     }
-    try:     # DRAM bytes per launch from the committed `ncu --set full` capture of the same kernels
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            ncu_traffic = json.load(f)
-    except Exception:
-        ncu_traffic = {}
     kernels = {}
     for k, b in alg.items():
         if k in stage:
             t_ms, calls = stage[k]
             kernels[k] = {"ms": t_ms, "calls": calls, "achieved_gbs": b / (t_ms * 1e-3) / 1e9,
-                          "frac_of_hbm_peak": b / (t_ms * 1e-3) / 1e9 / hbm, "algorithmic_bytes": b,
-                          "traffic": (ncu_traffic.get(k, {}).get("dram_bytes") if (n == 256 and args.ppc == 2) else None)}
+                          "frac_of_hbm_peak": b / (t_ms * 1e-3) / 1e9 / hbm, "algorithmic_bytes": b}
     dom = max((k for k in kernels), key=lambda k: kernels[k]["ms"] * kernels[k]["calls"])
     roofline = {"kernel": dom, "bound": "hbm", "achieved": kernels[dom]["achieved_gbs"], "peak": hbm, "unit": "GB/s",
-                "frac": kernels[dom]["frac_of_hbm_peak"], "traffic": kernels[dom]["traffic"], "peak_source": peak_src,
+                "frac": kernels[dom]["frac_of_hbm_peak"], "peak_source": HBM_PEAK_SOURCE,
                 "kernels": kernels,
                 "note": "stage durations from CUDA events recorded by the C++ driver inside the timed steps (a stage = "
                         "its main kernel plus the small ones it needs: stray / listed particles); gather_push and "
@@ -395,9 +434,9 @@ def run_engine(args):
                        "state": "steady state: %d untimed spin-up steps + %d warm-up steps before the timed region "
                                 "(the initial lattice has decayed into random in-cell positions)" % (args.spinup, args.warmup),
                        "use_filter": int(args.filter), "deposit_mode": int(args.deposit_mode), "gather_mode": int(args.gather_mode),
-                       "brick_grid": list(nb), "l2": "inputs (%.1f GB of particles per GPU) exceed the 126 MB L2"
+                       "brick_grid": list(nb), "l2": "inputs (%.1f GB of particles per GPU) exceed the 50 MB L2"
                                                      % (npart_local * 56 / 1e9)},
-            "e2e": e2e, "gpu_launches": launches, "clocks": clk, "roofline": roofline,
+            "e2e": e2e, "gpu_launches": launches, "device": device_info(local), "clocks": clk, "roofline": roofline,
             "stage_ms": {k: v[0] for k, v in stage.items()}, "stage_calls": {k: v[1] for k, v in stage.items()},
             "stage_sum_ms_per_step": step_sum, "host_enqueue_ms_per_step": 1e3 * t_host_enqueue / args.steps,
             "field_energy_J": list(fe), "host_generation_s": t_gen}
@@ -442,6 +481,9 @@ def main():
                     help="pic_set_deposit_mode: 0 register runs, 1 shared-memory tile block, 2 two lines per "
                          "lane, 3 per-slot reductions, 4 both, 5 four lines per lane, 6 four lines + per-slot reductions, "
                          "7 one lane per cell (every mode passes the parity tests)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what they computed as DIR/<name>.npy: the field energy, a "
+                         "seeded sample of every field component and of the particles (by id), float64, < 64 MB")
     ap.add_argument("--gather-mode", type=int, default=0, choices=[0, 1, 2, 3],
                     help="pic_set_gather_mode: 0 one particle per lane (default), 1 two particles of a cell per lane, "
                          "2 the same without the 128-register cap (A/B measurement; same parity tests)")
@@ -458,7 +500,9 @@ def main():
         run_reference(args)
     else:
         run_engine(args)
-    # the line is out and flushed; nothing below may hang the job (interpreter teardown of CUDA / NCCL state)
+    # the line is out and flushed.  The handlers registered with atexit still run (a profiler or tracer may have output
+    # to write); the interpreter's teardown of CUDA / NCCL state is skipped: nothing below may hang the job
+    atexit._run_exitfuncs()
     sys.stdout.flush()
     sys.stderr.flush()
     os._exit(0)

@@ -2,7 +2,7 @@
 // 62c2a81eac7862d526e5861ef2befc00b7f5b759, >= 24.10) -- TEST INFRASTRUCTURE ONLY.
 // It provides just enough of the AMReX vocabulary for a handful of WarpX *leaf* headers
 // (shape factors, pushers, FDTD stencil policies, constants) to be compiled VERBATIM from
-// /root/reference so that the oracle's restated arithmetic can be checked against the real
+// a WarpX source tree so that the oracle's restated arithmetic can be checked against the real
 // thing.  Double precision build (WarpX_PRECISION=DOUBLE, CMakeLists.txt:110,117).
 #ifndef SHIM_AMREX_REAL_H_
 #define SHIM_AMREX_REAL_H_

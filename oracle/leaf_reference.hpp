@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE -- the same Leaf interface as leaf_restated.hpp, but every routine
-// forwards to the REFERENCE's own header, compiled verbatim from /root/reference/Source through
-// the minimal AMReX stand-in in oracle/amrex_shim.  Only built where /root/reference exists
-// (oracle/Makefile target `ref` -> oracle/_ref/libpic_oracle_ref.so); no reference source is
+// forwards to the REFERENCE's own header, compiled verbatim from a WarpX source tree's Source/ through
+// the minimal AMReX stand-in in oracle/amrex_shim.  Only built on request
+// (make -C oracle ref REF=<WarpX tree> -> oracle/_ref/libpic_oracle_ref.so); no reference source is
 // copied into this repository.
 #ifndef PIC_ORACLE_LEAF_REFERENCE_HPP_
 #define PIC_ORACLE_LEAF_REFERENCE_HPP_

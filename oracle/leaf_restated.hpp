@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE -- CPU oracle, leaf arithmetic restated by hand.
 //
 // Each function restates one leaf routine of the reference (paths relative to
-// /root/reference/Source) with the SAME floating-point evaluation order, so that a build with
+// Source/ of ECP-WarpX/WarpX) with the SAME floating-point evaluation order, so that a build with
 // -ffp-contract=off is bit-identical to the reference headers compiled verbatim through
 // oracle/amrex_shim (see leaf_reference.hpp and tests/test_oracle_vs_reference_leaves.py).
 // Nothing outside tests/, __graft_entry__.smoke() and bench.py's CPU-baseline legs may use this.

@@ -6,7 +6,8 @@ this module.  The product package (warpx_b200/) never does.
 Two builds exist (oracle/Makefile):
   * ``restated``  -- leaf arithmetic restated by hand (oracle/libpic_oracle.so);
   * ``reference`` -- leaf arithmetic = the reference's own headers compiled verbatim
-                     (oracle/_ref/libpic_oracle_ref.so, built only where /root/reference exists).
+                     (oracle/_ref/libpic_oracle_ref.so, built only where WARPX_REFERENCE_DIR names a WarpX
+                     source tree; tests/golden/reference_leaves.json records what it computes).
 """
 import ctypes as C
 import os
@@ -23,10 +24,11 @@ _LIBS = {}
 
 
 def build(ref=True):
-    """Compile the oracle (and, where /root/reference exists, the reference-leaf variant)."""
+    """Compile the oracle (and, where WARPX_REFERENCE_DIR names a WarpX source tree, the reference-leaf variant)."""
     subprocess.run(["make", "-s", "-C", _HERE], check=True)
-    if ref and os.path.isdir("/root/reference/Source"):
-        subprocess.run(["make", "-s", "-C", _HERE, "ref"], check=True)
+    src = os.environ.get("WARPX_REFERENCE_DIR")
+    if ref and src and os.path.isdir(os.path.join(src, "Source")):
+        subprocess.run(["make", "-s", "-C", _HERE, "ref", "REF=" + os.path.abspath(src)], check=True)
 
 
 def have_ref():

@@ -3,10 +3,10 @@
 // FDTD run (Evolve/WarpXEvolve.cpp:93-347, 353-455, 473-531, 64-91).
 //
 // Built twice by oracle/Makefile:
-//   libpic_oracle.so           leaf arithmetic = hand restatement   (always; travels to the GPU box)
-//   _ref/libpic_oracle_ref.so  leaf arithmetic = reference headers compiled verbatim from
-//                              /root/reference through oracle/amrex_shim (only where the
-//                              reference tree exists; the built .so travels, sources do not)
+//   libpic_oracle.so           leaf arithmetic = hand restatement   (always)
+//   _ref/libpic_oracle_ref.so  leaf arithmetic = reference headers compiled verbatim from a
+//                              WarpX source tree through oracle/amrex_shim (on request:
+//                              make ref REF=<tree>; tests/golden/reference_leaves.json records it)
 #ifdef ORC_LEAF_REFERENCE
 #include "leaf_reference.hpp"
 using Leaf = orc::LeafReference;

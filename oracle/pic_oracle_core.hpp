@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE -- CPU oracle of the explicit EM-PIC step (fp64), templated on the leaf
 // arithmetic (leaf_restated.hpp = hand restatement, leaf_reference.hpp = reference headers
 // compiled verbatim).  Every routine cites the reference lines it follows (paths relative to
-// /root/reference/Source).  Loop order and accumulation order follow the reference's CPU path.
+// Source/ of ECP-WarpX/WarpX).  Loop order and accumulation order follow the reference's CPU path.
 //
 // Only tests/, __graft_entry__.smoke() and the cpu_baseline / --impl reference legs of bench.py
 // may use this; the product (warpx_b200/) never links, imports or executes anything in oracle/.

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE -- CPU oracle of the stages that the laser-wakefield decks add to the
 // periodic EM-PIC step (SURVEY.md 8f rank 3): PEC field / current boundaries, the moving window,
 // the laser antenna and continuous plasma injection.  fp64, single box covering the domain.
-// Every routine cites the reference lines it follows (paths relative to /root/reference/Source).
+// Every routine cites the reference lines it follows (paths relative to Source/ of ECP-WarpX/WarpX).
 //
 // Only tests/, __graft_entry__.smoke() and the cpu_baseline / --impl reference legs of bench.py
 // may use this; the product (warpx_b200/) never links, imports or executes anything in oracle/.

@@ -19,7 +19,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -35,6 +35,13 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(scope="session")
 def golden():
     with open(os.path.join(ROOT, "tests", "golden", "warpx_checksums.json")) as f:
+        return json.load(f)
+
+
+@pytest.fixture(scope="session")
+def reference_leaves():
+    """Digests of what the reference's own leaf headers compute on the seeded inputs of tests/helpers.py."""
+    with open(os.path.join(ROOT, "tests", "golden", "reference_leaves.json")) as f:
         return json.load(f)
 
 

@@ -1,6 +1,7 @@
 #!/usr/bin/env python3
-"""Regenerates tests/golden/warpx_checksums.json from the reference tree (run in the authoring
-container only; /root/reference does not exist on the GPU box).
+"""Regenerates tests/golden/warpx_checksums.json and nci_godfrey_lines.json from a WarpX source tree:
+
+    python tests/golden/make_golden.py <WarpX source tree>
 
 The values are WarpX's own regression checksums for the tests that pin the hot path
 (SURVEY.md section 8c): the 3D Langmuir wave (full loop, order 1), the force-free particle pusher and
@@ -9,8 +10,10 @@ window, the laser antenna and continuous injection -- no RNG in that deck).
 Nothing else is taken from the reference."""
 import json
 import os
+import sys
 
-REF = "/root/reference/Regression/Checksum/benchmarks_json"
+WARPX = sys.argv[1]
+REF = os.path.join(WARPX, "Regression", "Checksum", "benchmarks_json")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "warpx_checksums.json")
 
 gold = {
@@ -41,7 +44,7 @@ print("wrote", OUT)
 # (pic_apply_nci_filter), the tests need a handful of lines to check the restated interpolation.
 import re
 
-TABLES = "/root/reference/Source/Utils/NCIGodfreyTables.H"
+TABLES = os.path.join(WARPX, "Source", "Utils", "NCIGodfreyTables.H")
 OUT2 = os.path.join(os.path.dirname(os.path.abspath(__file__)), "nci_godfrey_lines.json")
 text = open(TABLES).read()
 tab_length = int(re.search(r"const int tab_length = (\d+);", text).group(1))

@@ -38,7 +38,7 @@ def build():
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     cmd = [NVCC, "-DPIC_HOST_HARNESS", "-O2", "-std=c++17", "-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC",
            "-Xcompiler", "-ffp-contract=off", "--fmad=false", "--expt-relaxed-constexpr",
-           "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", OUT] + \
+           "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", OUT] + \
           ["-I", CSRC] + [os.path.join(CSRC, f) for f in SRCS] + PROBES + ["-lcudart"]
     subprocess.run(cmd, check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
     return OUT

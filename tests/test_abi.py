@@ -1,4 +1,4 @@
-"""CPU tests: the C-ABI library builds for sm_100a, loads, and exports every symbol that
+"""CPU tests: the C-ABI library builds for sm_90a (H100), loads, and exports every symbol that
 include/pic_b200.h declares (no compute calls without a GPU)."""
 import ctypes as C
 import os
@@ -15,14 +15,20 @@ def declared_functions():
 
 def test_header_symbols_are_exported():
     from warpx_b200 import build
-    path = build.build()          # nvcc cross-compiles sm_100a without a GPU
+    path = build.build()          # nvcc cross-compiles sm_90a without a GPU
     L = C.CDLL(path)
     names = declared_functions()
     assert len(names) >= 18
     for n in names:
         assert hasattr(L, n), n
     L.pic_version.restype = C.c_char_p
-    assert b"sm_100a" in L.pic_version()
+    assert b"sm_90a" in L.pic_version()
+    # every device image in the library is sm_90a code (an image for another architecture does not load on an H100)
+    import subprocess
+    cuobjdump = os.path.join(os.path.dirname(build.NVCC), "cuobjdump")
+    elves = subprocess.run([cuobjdump, "--list-elf", path], capture_output=True, text=True, check=True).stdout.split()
+    cubins = [e for e in elves if e.endswith(".cubin")]
+    assert cubins and all(e.endswith(".sm_90a.cubin") for e in cubins), cubins
 
 
 def test_ctypes_mirror_matches_header_layout():
@@ -60,3 +66,17 @@ def test_product_never_imports_oracle():
                 txt = open(os.path.join(dirpath, f)).read()
                 assert not re.search(r"import\s+oracle|from\s+oracle|oracle/|oracle\.|libpic_oracle|orc_[a-z]", txt), \
                     os.path.join(dirpath, f)
+
+
+def test_library_is_current_by_content_not_by_time(monkeypatch):
+    """A copied or re-checked-out tree (new modification times) keeps using the library build() made; other sources
+    or flags make it stale."""
+    from warpx_b200 import build
+    build.build()
+    assert not build.stale()
+    later = os.path.getmtime(build.LIB) + 100
+    for f in build.sources():
+        os.utime(f, (later, later))
+    assert not build.stale()
+    monkeypatch.setattr(build, "digest", lambda: "0" * 64)
+    assert build.stale()

@@ -20,7 +20,7 @@ class _Event:
         return 2.0
 
 
-def test_bench_engine_arm_prints_one_complete_line(monkeypatch, capfd):
+def test_bench_engine_arm_prints_one_complete_line(monkeypatch, capfd, tmp_path):
     import torch
     from host_harness import harness
     import bench
@@ -42,9 +42,15 @@ def test_bench_engine_arm_prints_one_complete_line(monkeypatch, capfd):
     monkeypatch.setattr(Host, "enable_stage_timing", lambda self, on=True: None)
     monkeypatch.setattr(Host, "stage_ms", lambda self: {"gather_push": (1.0, 2), "deposit": (2.0, 2), "evolve_b": (0.1, 4),
                                                       "evolve_e": (0.1, 2), "sort": (0.5, 1)})
+    evolved = []
+    real_evolve = Host.Evolve
+    monkeypatch.setattr(Host, "Evolve", lambda self, n, **k: (evolved.append(n), real_evolve(self, n, **k))[1])
+    dump = tmp_path / "dump"
     monkeypatch.setattr(sys, "argv", ["bench.py", "--cells", "16", "--steps", "2", "--warmup", "3", "--spinup", "1",
-                                      "--cpu-cells", "16", "--cpu-steps", "1", "--deposit-mode", "7"])
+                                      "--cpu-cells", "16", "--cpu-steps", "1", "--deposit-mode", "7",
+                                      "--dump-outputs", str(dump)])
     monkeypatch.setattr(bench.os, "_exit", lambda code: (_ for _ in ()).throw(SystemExit(code)))
+    monkeypatch.setattr(bench.atexit, "_run_exitfuncs", lambda: None)      # not pytest's own exit handlers
     with pytest.raises(SystemExit) as e:
         bench.main()
     assert e.value.code == 0
@@ -59,6 +65,18 @@ def test_bench_engine_arm_prints_one_complete_line(monkeypatch, capfd):
     assert line["e2e"]["h2d_bytes_per_step"] > 0 and line["e2e"]["d2h_bytes_per_step"] == 16
     assert line["cpu_baseline"]["value"] and line["cpu_baseline"]["cores"] >= 1
     assert "workload" in line["config"] and line["config"]["deposit_mode"] == 7
+    assert evolved[:3] == [1, 3, 2]                  # spin-up, warm-up, then exactly --steps timed steps
+    # --dump-outputs: what the timed steps computed, float64, a fixed sample, well under 64 MB
+    import numpy as np
+    from warpx_b200 import abi
+    names = ["field_energy", "particle_id"] + list(abi.COMP_NAMES) + ["particle_" + k for k in ("x", "y", "z", "w", "ux", "uy", "uz")]
+    assert sorted(p.name for p in dump.iterdir()) == sorted(n + ".npy" for n in names)
+    arrs = {n: np.load(dump / (n + ".npy")) for n in names}
+    assert all(a.dtype == np.float64 for a in arrs.values())
+    assert sum(a.nbytes for a in arrs.values()) <= 64 << 20
+    assert np.allclose(arrs["field_energy"], line["field_energy_J"], rtol=1e-12)
+    assert arrs["Ex"].size == 16 * 17 * 17 and np.all(np.diff(arrs["particle_id"]) > 0)     # valid points, nodal in y, z
+    assert arrs["particle_x"].size == arrs["particle_id"].size == 16 ** 3 * 8
     harness.host_library().pic_set_deposit_mode(0)
 
 
@@ -66,6 +84,7 @@ def test_bench_reference_arm_prints_one_line(monkeypatch, capfd):
     import bench
     monkeypatch.setattr(sys, "argv", ["bench.py", "--impl", "reference", "--cpu-cells", "16", "--steps", "2", "--warmup", "1"])
     monkeypatch.setattr(bench.os, "_exit", lambda code: (_ for _ in ()).throw(SystemExit(code)))
+    monkeypatch.setattr(bench.atexit, "_run_exitfuncs", lambda: None)      # not pytest's own exit handlers
     with pytest.raises(SystemExit):
         bench.main()
     out = [ln for ln in capfd.readouterr().out.splitlines() if ln.startswith("{")]

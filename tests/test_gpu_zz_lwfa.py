@@ -5,7 +5,7 @@ against the oracle and against WarpX's own golden checksums (test_3d_laser_accel
 
 Tolerances: the thin kernels copy / negate / add values -> bit-exact; the laser profile uses
 exp / sincos of the device -> 1e-13 of the peak momentum; loops as in test_gpu_parity.py.
-(Sorts after test_gpu_parity.py.  Green on a B200: profiles/r1l_gpu_tests.txt.)"""
+(Sorts after test_gpu_parity.py.)"""
 import ctypes as C
 import math
 

@@ -418,28 +418,17 @@ def test_host_guard_cells_with_moving_window_match_oracle(orc):
 
 
 @pytest.mark.parametrize("order", [1, 2, 3, 4])
-def test_device_shape_factors_match_reference_leaves(orc, hh, order):
+def test_device_shape_factors_match_reference_leaves(orc, hh, order, reference_leaves):
     """The shape-factor templates the kernels use (pic_common.cuh, __host__ __device__) against the
-    reference's ShapeFactors.H compiled verbatim (oracle/_ref) -- or its restatement -- including the
-    order-4 spline and the shifted (old-position) factors of the Esirkepov scheme."""
-    L = orc.lib("reference" if orc.have_ref() else "restated")
-    rng = np.random.default_rng(60 + order)
-    xs = np.concatenate([rng.uniform(0.0, 40.0, 4000), np.arange(0, 12) * 1.0, np.arange(0, 12) + 0.5])
-    for x in xs:
-        a, b = (C.c_double * 8)(), (C.c_double * 8)()
-        ja, jb = hh.pic_host_shape(order, float(x), a), L.orc_shape(order, float(x), b)
-        assert ja == jb and list(a) == list(b), x
-        assert abs(sum(a) - 1.0) < 1e-14
-        for dxo in (-0.7, -0.2, 0.0, 0.3, 0.9):
-            x_old = float(x) + dxo
-            if x_old < 0:
-                continue
-            i_new = ja + {1: 0, 2: 1, 3: 1, 4: 2}[order]          # index of the new position's nearest/left node
-            i_new = hh.pic_host_shape(order, float(x), (C.c_double * 8)())
-            sa, sb = (C.c_double * 8)(), (C.c_double * 8)()
-            ia = hh.pic_host_shifted_shape(order, x_old, i_new, sa)
-            ib = L.orc_shifted_shape(order, x_old, i_new, sb)
-            assert ia == ib and list(sa) == list(sb), (x, x_old)
+    reference's ShapeFactors.H compiled verbatim (digests of what oracle/_ref computed on the same positions),
+    including the order-4 spline and the shifted (old-position) factors of the Esirkepov scheme."""
+    from helpers import digest, shape_factor_outputs
+    got = shape_factor_outputs(order, hh.pic_host_shape, hh.pic_host_shifted_shape)
+    for row in got["shape"]:
+        assert abs(sum(row[1:]) - 1.0) < 1e-14, row
+    want = reference_leaves["shape_factors"][str(order)]
+    for k in ("shape", "shifted_shape"):
+        assert digest(got[k]) == want[k], k
 
 
 # ---------------------------------------------------------------------------------------------

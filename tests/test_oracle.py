@@ -1,5 +1,6 @@
-"""CPU tests (-m "not gpu"): the oracle against the reference's golden vectors and against the
-reference's own leaf headers; host logic of the decomposition."""
+"""CPU tests (-m "not gpu"): the oracle against the reference's golden vectors and against what the
+reference's own leaf headers compute (digests in tests/golden/reference_leaves.json); host logic of the
+decomposition."""
 import ctypes as C
 import math
 
@@ -90,89 +91,28 @@ def test_particle_pusher_known_answer(orc, golden, pusher, name):
         assert _close(abs(u[1] * m), g["particle_momentum_y"], 1e-9)
 
 
-def test_restated_leaves_match_reference_headers_bitwise(orc):
-    """The hand-restated leaf arithmetic vs the reference's own headers compiled verbatim
-    (oracle/_ref): identical bits on shape factors, pushers, stencil coefficients and dt."""
-    if not orc.have_ref():
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
-    A, B = orc.lib("restated"), orc.lib("reference")
-    assert A.orc_leaf_name() == b"restated" and B.orc_leaf_name() == b"reference"
-    rng = np.random.default_rng(7)
-    for order in range(0, 5):
-        for x in rng.uniform(0.0, 40.0, 400):
-            sa, sb = (C.c_double * 8)(), (C.c_double * 8)()
-            assert A.orc_shape(order, x, sa) == B.orc_shape(order, x, sb)
-            assert list(sa) == list(sb)
-            i_new = A.orc_shape(order, x, sa)
-            xo = x + rng.uniform(-0.999, 0.999)
-            sa, sb = (C.c_double * 8)(), (C.c_double * 8)()
-            assert A.orc_shifted_shape(order, xo, i_new, sa) == B.orc_shifted_shape(order, xo, i_new, sb)
-            assert list(sa) == list(sb)
-    for pusher in (0, 1, 2):
-        for _ in range(300):
-            u0 = rng.normal(0, 3e8, 3)
-            eb = np.concatenate([rng.normal(0, 1e11, 3), rng.normal(0, 300.0, 3)])
-            ua, ub = (C.c_double * 3)(*u0), (C.c_double * 3)(*u0)
-            ebc = (C.c_double * 6)(*eb)
-            A.orc_push_momentum(pusher, ua, ebc, -workloads.Q_E, workloads.M_E, 1.3e-16)
-            B.orc_push_momentum(pusher, ub, ebc, -workloads.Q_E, workloads.M_E, 1.3e-16)
-            assert list(ua) == list(ub)
-            xa, xb = (C.c_double * 3)(1e-6, 2e-6, 3e-6), (C.c_double * 3)(1e-6, 2e-6, 3e-6)
-            A.orc_update_position(xa, ua, 1.3e-16)
-            B.orc_update_position(xb, ub, 1.3e-16)
-            assert list(xa) == list(xb)
-    for algo in (0, 1):
-        for dx in ([1e-6, 1e-6, 1e-6], [1e-6, 2e-6, 0.5e-6]):
-            sa, sb = abi.pic_stencil(), abi.pic_stencil()
-            dxc = (C.c_double * 3)(*dx)
-            A.orc_stencil_coefs(algo, dxc, C.byref(sa))
-            B.orc_stencil_coefs(algo, dxc, C.byref(sb))
-            assert list(sa.cx) == list(sb.cx) and list(sa.cy) == list(sb.cy) and list(sa.cz) == list(sb.cz)
-            assert A.orc_max_dt(algo, dxc) == B.orc_max_dt(algo, dxc)
+def _assert_matches_reference(got, want):
+    """got: {name: array}; want: {name: SHA-256} recorded with the reference's headers (helpers.digest)."""
+    from helpers import digest
+    assert sorted(got) == sorted(want)
+    for k in sorted(got):
+        assert digest(got[k]) == want[k], k
 
 
-def test_restated_stages_match_reference_headers_bitwise(orc):
-    """Whole stages (FDTD Yee/CKC, gather+push, deposition) with restated vs reference leaves."""
-    if not orc.have_ref():
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
-    from helpers import random_fields, lower_corner
-    A, B = orc.lib("restated"), orc.lib("reference")
-    n = 12
-    box_lo, box_hi = (0, 0, 0), (n - 1,) * 3
-    prob_lo, prob_hi = (-1e-5,) * 3, (1e-5,) * 3
-    dx = [(prob_hi[d] - prob_lo[d]) / n for d in range(3)]
-    A.orc_set_num_threads(1); B.orc_set_num_threads(1)
-    for algo in (0, 1):
-        st = abi.pic_stencil()
-        A.orc_stencil_coefs(algo, (C.c_double * 3)(*dx), C.byref(st))
-        res = []
-        for L in (A, B):
-            F = random_fields(orc, box_lo, box_hi, (2, 2, 2), 3, comps=range(9), scale=[1e9] * 3 + [3.0] * 3 + [1e12] * 3)
-            E, Bf, J = orc.fab_array(F[0:3]), orc.fab_array(F[3:6]), orc.fab_array(F[6:9])
-            L.orc_evolve_b(Bf, E, C.byref(st), 1e-15)
-            L.orc_evolve_e(E, Bf, J, C.byref(st), 2e-15)
-            res.append([f.a.copy() for f in F])
-        for a, b in zip(*res):
-            assert np.array_equal(a, b)
-    wl = workloads.uniform_plasma_3d(n_cell=(n, n, n), ppc=(2, 1, 1), u_th=0.2, lx=2e-5)
-    sp = wl["species"][0]
-    for nox in (1, 2, 3):
-        ngEB = (4, 4, 4)
-        xyzmin, lo = lower_corner(prob_lo, dx, box_lo, ngEB)
-        dinv = [1.0 / v for v in dx]
-        res = []
-        for L in (A, B):
-            F = random_fields(orc, box_lo, box_hi, ngEB, 5, comps=range(9), scale=[1e10] * 3 + [30.0] * 3 + [0.0] * 3)
-            P = orc.HostParticles(**{k: sp[k] for k in orc.HostParticles.NAMES})
-            for pusher in (0, 1, 2):
-                L.orc_gather_push(C.byref(P.soa), 0, P.np, orc.fab_array(F[0:3]), orc.fab_array(F[3:6]),
-                                  abi.dbl3(dinv), abi.dbl3(xyzmin), abi.int3(lo), sp["q"], sp["m"], 2e-15,
-                                  nox, 1, pusher, 1)
-            L.orc_deposit_esirkepov(C.byref(P.soa), 0, P.np, orc.fab_array(F[6:9]), abi.dbl3(dinv),
-                                    abi.dbl3(xyzmin), abi.int3(lo), sp["q"], 2e-15, -1e-15, nox)
-            res.append([P.x.copy(), P.ux.copy(), P.uz.copy()] + [f.a.copy() for f in F[6:9]])
-        for a, b in zip(*res):
-            assert np.array_equal(a, b)
+def test_restated_leaves_match_reference_headers_bitwise(orc, reference_leaves):
+    """The hand-restated leaf arithmetic vs the reference's own headers compiled verbatim (digests of what
+    oracle/_ref computed on the same seeded inputs, tests/golden/reference_leaves.json): identical bits on shape
+    factors, pushers, stencil coefficients and dt."""
+    from helpers import leaf_outputs
+    A = orc.lib("restated")
+    assert A.orc_leaf_name() == b"restated"
+    _assert_matches_reference(leaf_outputs(orc, A), reference_leaves["leaves"])
+
+
+def test_restated_stages_match_reference_headers_bitwise(orc, reference_leaves):
+    """Whole stages (FDTD Yee/CKC, gather+push, deposition) with restated leaves vs the reference's digests."""
+    from helpers import stage_outputs
+    _assert_matches_reference(stage_outputs(orc, orc.lib("restated")), reference_leaves["stages"])
 
 
 def test_decomposition_independence_of_oracle(orc):
@@ -658,24 +598,16 @@ def test_particle_energy_known_answer_and_conservation(orc):
     assert abs((k1 + e1) - k0) <= 0.05 * k0        # ... and the total is conserved to a few per cent at 16^3
 
 
-def test_order4_oracle_identity_and_leaf_agreement(orc):
+def test_order4_oracle_identity_and_leaf_agreement(orc, reference_leaves):
     """algo.particle_shape = 4 (Source/WarpX.cpp:1307-1316): the Esirkepov identity sum J dV = sum q w v
     holds for the order-4 stencil, a 6-step loop runs with the guard cells guardCellManager gives
-    (ng_EB 4, ng_J 5), and the restated leaves agree with the reference's headers bit for bit."""
+    (ng_EB 4, ng_J 5), and the restated leaves agree with the reference's headers bit for bit (digests)."""
     wl = workloads.uniform_plasma_3d(n=12, ppc=(2, 1, 2), u_th=0.3, lx=3e-6, perturbation=0.02)
     s = wl["species"][0]
-    kinds = ["restated"] + (["reference"] if orc.have_ref() else [])
-    fields = []
-    for kind in kinds:
-        sim = orc.OracleSim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=4, kind=kind)
-        assert sim.guards() == {"ng_EB": [4, 4, 4], "ng_J": [5, 5, 5], "ng_FG": [2, 2, 2], "ng_FS": [1, 1, 1]}
-        sim.add_species(s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
-        sim.evolve(6)
-        fields.append([sim.fab(c)[1].copy() for c in range(9)])
-        assert all(np.isfinite(f).all() for f in fields[-1]) and np.max(np.abs(fields[-1][0])) > 0
-    if len(fields) == 2:
-        for a, b in zip(*fields):
-            assert np.array_equal(a, b)
+    from helpers import order4_loop_fields
+    fields = order4_loop_fields(orc, "restated")
+    assert all(np.isfinite(f).all() for f in fields.values()) and np.max(np.abs(fields["Ex"])) > 0
+    _assert_matches_reference(fields, reference_leaves["order4_loop"])
     # stage-level identity
     L = orc.lib()
     n = wl["n_cell"]

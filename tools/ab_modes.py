@@ -4,7 +4,7 @@ generated and uploaded once): for every deposition variant (pic_set_deposit_mode
 (pic_set_gather_mode 0..2) the per-stage times of the step (CUDA events around every stage, Python sequencer)
 and the whole-step time of the C++ driver.  Not a bench value -- a ranking tool for a scarce GPU slot:
 
-    gpurun --timeout 900 -- 'python tools/ab_modes.py --cells 256 > gpurun_out/ab_modes.json'
+    python tools/ab_modes.py --cells 256 > ab_modes.json
 
 Every variant passes the same parity tests (tests/test_gpu_zz_lwfa.py::test_deposit_variants_match_oracle,
 ::test_gather_variants_match_oracle); this script only times them."""
@@ -140,7 +140,7 @@ def main():
     best_g = min((v for v in out["variants"][:-1] if v["deposit_mode"] == 0), key=lambda v: v["ms_per_step"])
     out["best"] = {"deposit_mode": best_d["deposit_mode"], "gather_mode": best_g["gather_mode"]}
     print(json.dumps(out, indent=1))
-    # the same, compact, for the tail of a gpurun log (stderr, so that stdout stays one JSON document)
+    # the same, compact, for the tail of a log (stderr, so that stdout stays one JSON document)
     for v in out["variants"]:
         st = v.get("stage_ms", {})
         print("deposit_mode %d gather_mode %d : %7.2f ms/step   gather %6.2f  deposit %6.2f" %

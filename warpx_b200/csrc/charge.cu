@@ -1,7 +1,7 @@
 // Charge deposition and the PEC / reflecting boundary of rho -- the `rho` diagnostic of a plotfile
 // (outside the per-step path of the explicit FDTD loop: WarpX deposits rho only for diagnostics there).
 //
-// Replaces (paths relative to /root/reference/Source):
+// Replaces (paths relative to Source/ of ECP-WarpX/WarpX):
 //   pic_deposit_charge  <- WarpXParticleContainer::DepositCharge (Particles/WarpXParticleContainer.cpp:890-1216)
 //                          -> doChargeDepositionShapeN<N> (Particles/Deposition/ChargeDeposition.H:37-157)
 //   pic_apply_pec_rho   <- PEC::ApplyReflectiveBoundarytoRhofield (BoundaryConditions/WarpX_PEC.cpp:624-699)

@@ -12,7 +12,7 @@
 //    reduced in registers by a warp whose lanes own stencil lines; retired planes go to J with
 //    fp64 L2 reductions (~7 per particle instead of 540).
 //  * deposit_tile.cu (pic_set_deposit_mode(PIC_DEPOSIT_TILE)) -- same reduction, staged through a shared-memory J block
-//    per supercell; kept for comparison (slower on sm_100a: shared fp64 atomics are CAS loops).
+//    per supercell; kept for comparison (slower on sm_90a: shared fp64 atomics are CAS loops).
 #include "pic_common.cuh"
 #include "deposit_common.cuh"
 

@@ -21,7 +21,7 @@
 //       Particles that changed cell are appended to a list.
 //   deposit_general_kernel -- the listed particles with the full (N+3)^2 x (N+2) stencil.
 // Retired sums go to J with fp64 red.global (L2 reductions, no return value, no shared-memory
-// staging: on sm_100a shared fp64 atomics are CAS loops and the staging block would cap the SM at
+// staging: on sm_90a shared fp64 atomics are CAS loops and the staging block would cap the SM at
 // 8 resident warps -- measured in profiles/, see DESIGN.md).  Any particle order is CORRECT (a run
 // may be a single particle); cell-sorted order is FAST.
 #include "pic_common.cuh"

@@ -1,7 +1,7 @@
 // C++ host driver of the PIC step: the sequence of WarpX::Evolve / OneStep_nosub for a single-level,
 // periodic, explicit FDTD run on ONE rank, expressed as calls through the C ABI of this library.
 //
-// Mirrors (paths relative to /root/reference/Source):
+// Mirrors (paths relative to Source/ of ECP-WarpX/WarpX):
 //   pic_engine_evolve            <- WarpX::Evolve                          Evolve/WarpXEvolve.cpp:93-347
 //   explicit_fill_boundary_eb    <- ExplicitFillBoundaryEBUpdateAux        :473-531
 //   one_step_nosub               <- WarpX::OneStep_nosub                   :353-455

@@ -2,7 +2,7 @@
 // of BASELINE.json needs all of them): PEC walls on E, B and J, the moving-window shift, the laser
 // antenna, continuous plasma injection, absorbing / reflecting particle boundaries.
 //
-// Replaces (paths relative to /root/reference/Source):
+// Replaces (paths relative to Source/ of ECP-WarpX/WarpX):
 //   pic_apply_pec_field          <- PEC::ApplyPECtoEfield / ApplyPECtoBfield   BoundaryConditions/WarpX_PEC.cpp:456-612
 //   pic_apply_pec_current        <- PEC::ApplyReflectiveBoundarytoJfield       BoundaryConditions/WarpX_PEC.cpp:702-880
 //   pic_shift_fab                <- WarpX::shiftMF                             Utils/WarpXMovingWindow.cpp:478-604

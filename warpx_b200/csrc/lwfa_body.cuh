@@ -5,7 +5,7 @@
 // that tests/host_harness can run the SAME code over the same index space on the host (a check of
 // the per-thread logic where no GPU is available; never part of the product path).
 //
-// Reference (paths relative to /root/reference/Source):
+// Reference (paths relative to Source/ of ECP-WarpX/WarpX):
 //   pec_field_body        <- ::SetEfieldOnPEC / ::SetBfieldOnPEC     BoundaryConditions/WarpX_PEC.cpp:120-190,252-318
 //   pec_current_body      <- ::SetRhoOrJfieldFromPEC                 BoundaryConditions/WarpX_PEC.cpp:340-395
 //   shift_body            <- WarpX::shiftMF                          Utils/WarpXMovingWindow.cpp:508-600

@@ -1,7 +1,7 @@
 // Godfrey's numerical-Cherenkov corrector (particles.use_fdtd_nci_corr): a 5-point filter along z applied
 // to a COPY of E and B that the field gather reads instead of the fields themselves.
 //
-// Replaces (paths relative to /root/reference/Source):
+// Replaces (paths relative to Source/ of ECP-WarpX/WarpX):
 //   pic_nci_godfrey_table_index / pic_nci_godfrey_stencil
 //        <- NCIGodfreyFilter::ComputeStencils                      Filter/NCIGodfreyFilter.cpp:49-139
 //   pic_apply_nci_filter

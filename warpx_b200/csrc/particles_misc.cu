@@ -186,7 +186,7 @@ extern "C" int pic_particles_wrap_listed(const pic_soa* p, const pic_geom* g, co
         wg.lo[d] = g->prob_lo[d]; wg.hi[d] = g->prob_hi[d]; wg.len[d] = g->prob_hi[d] - g->prob_lo[d];
         wg.periodic[d] = g->periodic[d];
     }
-    wrap_listed_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(make_soa(*p, 0), p->np, wg, e->idx, e->count, e->capacity);
+    wrap_listed_kernel<<<NUM_SMS * 8, 256, 0, (cudaStream_t)stream>>>(make_soa(*p, 0), p->np, wg, e->idx, e->count, e->capacity);
     count_launch();
     return check_launch("pic_particles_wrap_listed") ? 0 : 1;
 }
@@ -216,7 +216,7 @@ extern "C" int pic_particles_classify_listed(const pic_soa* p, const pic_geom* g
     if (p->np == 0) return 0;
     const double* pos = dim == 0 ? p->x : (dim == 1 ? p->y : p->z);
     const double dinv = 1.0 / ((g->prob_hi[dim] - g->prob_lo[dim]) / g->n_cell[dim]);
-    classify_listed_kernel<<<148 * 8, 256, 0, s>>>(pos, p->np, np_dev, g->prob_lo[dim], dinv, g->n_cell[dim], cell_lo, cell_hi,
+    classify_listed_kernel<<<NUM_SMS * 8, 256, 0, s>>>(pos, p->np, np_dev, g->prob_lo[dim], dinv, g->n_cell[dim], cell_lo, cell_hi,
                                                    both_up, counts, idx_lo, idx_hi, capacity, cand->idx, cand->count,
                                                    cand->capacity);
     count_launch();

@@ -1,4 +1,4 @@
-// Shared device/host helpers of the B200 PIC kernels (sm_100a only; no multi-arch paths).
+// Shared device/host helpers of the PIC kernels (sm_90a, H100, only; no multi-arch paths).
 #ifndef PIC_COMMON_CUH_
 #define PIC_COMMON_CUH_
 
@@ -16,7 +16,7 @@ constexpr double MU0 = 1.25663706212e-06;
 constexpr double EP0 = 8.8541878128e-12;
 constexpr double INV_C2 = 1.0 / (C_LIGHT * C_LIGHT);
 
-constexpr int NUM_SMS = 148;  // B200: 2 dies x 74 SMs
+constexpr int NUM_SMS = 132;  // H100 SXM
 
 // ---- error handling (mirrors amrex::Abort unless tests ask for return codes) ---------------
 int fail(const char* fmt, ...);

@@ -37,5 +37,5 @@ bool check_launch(const char* what) {
 
 extern "C" void pic_set_error_mode(int mode) { pic::g_error_mode = mode; }
 extern "C" const char* pic_last_error(void) { return pic::g_last_error; }
-extern "C" const char* pic_version(void) { return "pic_b200 0.1 (sm_100a, fp64)"; }
+extern "C" const char* pic_version(void) { return "pic_b200 0.1 (sm_90a, fp64)"; }
 extern "C" long pic_launch_count(void) { return pic::g_launches.load(); }

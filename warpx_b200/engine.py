@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's explicit EM-PIC step (single level, periodic, FDTD).
 
 Method names, argument meaning and sequencing follow WarpX so that the parity tests read like the
-reference (paths relative to /root/reference/Source):
+reference (paths relative to Source/ of ECP-WarpX/WarpX):
 
     Simulation.Evolve                     <- WarpX::Evolve                     Evolve/WarpXEvolve.cpp:93-347
     Simulation.ExplicitFillBoundaryEBUpdateAux                                 :473-531
@@ -14,7 +14,7 @@ reference (paths relative to /root/reference/Source):
     Simulation.Synchronize                <- WarpX::Synchronize                Evolve/WarpXEvolve.cpp:64-91
     Simulation.HandleParticlesAtBoundaries                                     :533-581
 
-Every stage is one call through the C ABI (include/pic_b200.h) into hand-written sm_100a kernels;
+Every stage is one call through the C ABI (include/pic_b200.h) into hand-written sm_90a kernels;
 PyTorch only owns device memory, the stream and (multi-GPU) the NCCL transport.
 There is no CPU path: constructing a Simulation without a CUDA device raises.
 """

@@ -1,7 +1,7 @@
 """Loader of the C-ABI shared library (warpx_b200/libpic_b200.so).
 
-There is no CPU fallback: if the library is missing it is built with nvcc (sm_100a cross-compiles
-without a GPU); if that fails, or a kernel is requested without a CUDA device, the call raises.
+There is no CPU fallback: if the library is missing, or was built from other sources, it is built with nvcc (sm_90a
+cross-compiles without a GPU); if that fails, or a kernel is requested without a CUDA device, the call raises.
 """
 import ctypes as C
 import os
@@ -16,22 +16,31 @@ def lib():
     if _LIB is not None:
         return _LIB
     path = _build.LIB
-
-    def needs_build():
-        return not os.path.exists(path) or (os.path.isdir(_build.CSRC) and _build.stale() and os.path.exists(_build.NVCC))
-    if needs_build():
-        # one process per GPU: only one rank compiles, the others wait for the lock and find the library fresh
-        import fcntl
-        with open(os.path.join(_build.HERE, ".build.lock"), "w") as lock:
-            fcntl.flock(lock, fcntl.LOCK_EX)
-            try:
-                if needs_build():
-                    path = _build.build()
-            finally:
-                fcntl.flock(lock, fcntl.LOCK_UN)
+    if not os.path.exists(path) or (os.path.isdir(_build.CSRC) and os.path.exists(_build.NVCC) and _build.stale()):
+        path = _rebuild()
     _LIB = bind(C.CDLL(path))
     _LIB.pic_apply_env_defaults()
     return _LIB
+
+
+def _rebuild():
+    """Build the library from the current sources: in-tree when the package directory is writable, otherwise (a
+    read-only install) into a per-user directory under the system's temporary directory, never into the tree."""
+    import fcntl
+    import tempfile
+    if os.access(_build.HERE, os.W_OK):
+        where, target = _build.HERE, _build.LIB
+    else:
+        where = os.path.join(tempfile.gettempdir(), "warpx_b200-%d" % os.getuid(), _build.digest()[:16])
+        os.makedirs(where, exist_ok=True)
+        target = os.path.join(where, os.path.basename(_build.LIB))
+    # one process per GPU: only one rank compiles, the others wait for the lock and find the library fresh
+    with open(os.path.join(where, ".build.lock"), "w") as lock:
+        fcntl.flock(lock, fcntl.LOCK_EX)
+        try:
+            return _build.build(lib=target)
+        finally:
+            fcntl.flock(lock, fcntl.LOCK_UN)
 
 
 def bind(L):
@@ -128,7 +137,7 @@ def bind(L):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise RuntimeError("warpx_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("warpx_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return torch
 
 
