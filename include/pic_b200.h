@@ -230,13 +230,16 @@ int pic_deposit_esirkepov(const pic_soa* p, long offset, long np,
  * PIC_DEPOSIT_RUNS_SLOTRED / PIC_DEPOSIT_RUNS2_SLOTRED: the particle slots of a warp pass send their own
  *   partial sums to L2 instead of being summed by shuffles first.
  * PIC_DEPOSIT_RUNS4 / PIC_DEPOSIT_RUNS4_SLOTRED: four lines per lane (order 3 only; 168 registers).
+ * PIC_DEPOSIT_RUNS_SLAB: PIC_DEPOSIT_RUNS retiring into a per-warp shared-memory J slab (lone strays too), added to
+ *   J with coalesced L2 reductions at a rebase and at the end of the warp's particles (orders 1..3).
  * Modes 2..6 are experiments until measured; all pass the same parity tests.
  * Analogous to WarpX's runtime switch warpx.do_shared_mem_current_deposition
  * (Source/WarpX.cpp:126, Docs/source/usage/parameters.rst:2608-2623). */
 enum { PIC_DEPOSIT_RUNS = 0, PIC_DEPOSIT_TILE = 1, PIC_DEPOSIT_RUNS2 = 2, PIC_DEPOSIT_RUNS_SLOTRED = 3,
        PIC_DEPOSIT_RUNS2_SLOTRED = 4, PIC_DEPOSIT_RUNS4 = 5, PIC_DEPOSIT_RUNS4_SLOTRED = 6, PIC_DEPOSIT_CELLS = 7,
        PIC_DEPOSIT_CELLS2 = 8, PIC_DEPOSIT_CELLS2_WIDE = 9 /* lane per cell with two producer warps (3 / 2 CTAs per SM) */,
-       PIC_DEPOSIT_CELLS3 = 10, PIC_DEPOSIT_CELLS3_WIDE = 11 /* the same, producers and consumers decoupled by mbarriers */ };
+       PIC_DEPOSIT_CELLS3 = 10, PIC_DEPOSIT_CELLS3_WIDE = 11 /* the same, producers and consumers decoupled by mbarriers */,
+       PIC_DEPOSIT_RUNS_SLAB = 12 };
 void pic_set_deposit_mode(int mode);
 
 /* ------------------------------------------------------------------------------------------

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """A/B of the experimental kernel variants on the benchmark workload, in ONE process (the 256^3 x 8 ppc state is
-generated and uploaded once): for every deposition variant (pic_set_deposit_mode 0..6) and gather variant
+generated and uploaded once): for every deposition variant (pic_set_deposit_mode 0..7, 12) and gather variant
 (pic_set_gather_mode 0..2) the per-stage times of the step (CUDA events around every stage, Python sequencer)
 and the whole-step time of the C++ driver.  Not a bench value -- a ranking tool for a scarce GPU slot:
 
@@ -27,7 +27,7 @@ def main():
                     "(64 spin-up steps, then 16 timed), default kernels")
     ap.add_argument("--fresh", action="store_true", help="a new Simulation per variant: stage times on the FRESH state "
                     "(steps 4..12 after the upload) instead of one long-running state")
-    ap.add_argument("--deposit-modes", default="0,7,2,5,6")
+    ap.add_argument("--deposit-modes", default="0,12,7,2,5,6")
     ap.add_argument("--gather-modes", default="0,1,2,3")
     args = ap.parse_args()
     import torch

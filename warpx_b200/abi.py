@@ -143,6 +143,7 @@ PUSHER_BORIS, PUSHER_VAY, PUSHER_HC = 0, 1, 2
 # pic_set_deposit_mode / pic_set_gather_mode (include/pic_b200.h)
 PIC_DEPOSIT_RUNS, PIC_DEPOSIT_TILE, PIC_DEPOSIT_CELLS, PIC_DEPOSIT_CELLS2, PIC_DEPOSIT_CELLS2_WIDE = 0, 1, 7, 8, 9
 PIC_DEPOSIT_CELLS3, PIC_DEPOSIT_CELLS3_WIDE = 10, 11
+PIC_DEPOSIT_RUNS_SLAB = 12
 PIC_GATHER_TILE, PIC_GATHER_PAIRS, PIC_GATHER_PAIRS_WIDE = 0, 1, 2
 
 # Yee staggering of WarpX (Source/WarpX.cpp:2117-2125): 1 = nodal.  Order Ex Ey Ez Bx By Bz jx jy jz.

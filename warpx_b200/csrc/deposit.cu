@@ -10,7 +10,8 @@
 //    drop-in for callers that cannot provide cell bins.
 //  * deposit_runs.cu (default with bins) -- cell-sorted particles: runs of same-cell particles are
 //    reduced in registers by a warp whose lanes own stencil lines; retired planes go to J with
-//    fp64 L2 reductions (~7 per particle instead of 540).
+//    fp64 L2 reductions (~7 per particle instead of 540).  PIC_DEPOSIT_RUNS_SLAB retires them into a
+//    per-warp shared-memory J slab first (slower on the H100, DESIGN.md 3.3).
 //  * deposit_tile.cu (pic_set_deposit_mode(PIC_DEPOSIT_TILE)) -- same reduction, staged through a shared-memory J block
 //    per supercell; kept for comparison (slower on sm_90a: shared fp64 atomics are CAS loops).
 #include "pic_common.cuh"
@@ -90,7 +91,8 @@ extern "C" void pic_set_deposit_mode(int mode) {
     g_cells_two_producers = (mode >= PIC_DEPOSIT_CELLS2 && mode <= PIC_DEPOSIT_CELLS3_WIDE) ? mode - PIC_DEPOSIT_CELLS2 + 1 : 0;
     if (g_cells_two_producers) g_deposit_mode = PIC_DEPOSIT_CELLS;
     g_runs_variant = (mode == PIC_DEPOSIT_RUNS2) ? 1 : (mode == PIC_DEPOSIT_RUNS_SLOTRED) ? 2 : (mode == PIC_DEPOSIT_RUNS2_SLOTRED) ? 3
-                   : (mode == PIC_DEPOSIT_RUNS4) ? 4 : (mode == PIC_DEPOSIT_RUNS4_SLOTRED) ? 6 : 0;
+                   : (mode == PIC_DEPOSIT_RUNS4) ? 4 : (mode == PIC_DEPOSIT_RUNS4_SLOTRED) ? 6
+                   : (mode == PIC_DEPOSIT_RUNS_SLAB) ? 8 : 0;
 }
 
 extern "C" int pic_deposit_esirkepov(const pic_soa* p, long offset, long np, const pic_fab J[3],

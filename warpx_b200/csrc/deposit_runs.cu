@@ -20,10 +20,16 @@
 //       reductions per cell instead of the reference's (N+2)(N+3)^2*3 = 540 per PARTICLE.
 //       Particles that changed cell are appended to a list.
 //   deposit_general_kernel -- the listed particles with the full (N+3)^2 x (N+2) stencil.
-// Retired sums go to J with fp64 red.global (L2 reductions, no return value, no shared-memory
-// staging: on sm_90a shared fp64 atomics are CAS loops and the staging block would cap the SM at
-// 8 resident warps -- measured in profiles/, see DESIGN.md).  Any particle order is CORRECT (a run
-// may be a single particle); cell-sorted order is FAST.
+// Retired sums go to J with fp64 red.global (L2 reductions, no return value).  PIC_DEPOSIT_RUNS_SLAB (ZS > 0
+// below) retires them into a per-warp shared-memory J slab instead: one supercell's 8 x 8 cells
+// in x, y and ZS cell layers in z, grown by the stencil reach.  A warp's 512 particles cover about 64
+// cells -- one z layer of a supercell -- so the slab is rebased rarely; a rebase and the end of the
+// warp's span add the slab to J with fp64 red.global along x rows, zeros skipped.  The slab takes plain
+// read-modify-writes: its one writer is the warp, inside one retire instruction the sender lanes own
+// distinct lines and so touch distinct nodes, and retires are ordered by __syncwarp (no shared fp64
+// atomicAdd: on sm_90a that is a CAS loop).  On the H100 the slab variant is slower (DESIGN.md section
+// 3.3): the slab halves the resident warps and a shared read-modify-write waits where red.global does
+// not.  Any particle order is CORRECT (a run may be a single particle); cell-sorted order is FAST.
 #include "pic_common.cuh"
 #include "deposit_common.cuh"
 #ifdef PIC_SIMT_HOST
@@ -33,12 +39,30 @@
 namespace pic {
 
 // bit 0: two v-lines per lane where N+1 is even; bit 1: per-slot reductions instead of the shuffle fold;
-// bit 2: four v-lines per lane (order 3 only; 168 registers -> 3 CTAs of 4 warps per SM)
+// bit 2: four v-lines per lane (order 3 only; 168 registers -> 3 CTAs of 4 warps per SM); bit 3: the J slab
 int g_runs_variant = 0;
 
 constexpr int DR_CH = 32;          // particles per chunk
 constexpr int DR_CHP = DR_CH + 1;  // record pitch (odd: conflict-free column access)
 constexpr unsigned FULL = 0xffffffffu;
+
+#ifdef PIC_DEPOSIT_COUNTERS
+// What the quiet kernel does, counted under the host emulator (tests/host_harness, one OS thread); the
+// library build never defines PIC_DEPOSIT_COUNTERS.
+struct RunsCounters {
+    long chunks, particles, movers, runs, slides, jumps, lones, lones_outside, rebases, cells;
+    long red_retire, red_lone, red_slab;      // fp64 reductions sent to J by the three paths
+};
+RunsCounters g_runs_counters;
+#define DR_COUNT(field, v) (::pic::g_runs_counters.field += (v))
+extern "C" void pic_runs_counters(long* out, int reset) {     // the fields in declaration order
+    constexpr int n = sizeof(RunsCounters) / sizeof(long);
+    for (int i = 0; i < n; ++i) out[i] = reinterpret_cast<const long*>(&g_runs_counters)[i];
+    if (reset) g_runs_counters = RunsCounters{};
+}
+#else
+#define DR_COUNT(field, v) ((void)0)
+#endif
 
 // ---- per-direction weights without dynamic indexing -------------------------------------------
 // shifted (old-position) weights: slot s holds w[s-1-sh], sh in {-1,0,1}  (ShapeFactors.H:93-156)
@@ -85,20 +109,33 @@ __device__ __forceinline__ long fab_stride(const FabView& F, int d) { return d =
 
 // SLOTRED = true: the NG particle slots of a pass are not summed by shuffles before a plane is retired --
 // every slot sends its own partial sums to L2 (NG times the reductions, no SHFL; experiment).
-template <int N, int NW, int MINB, int R0, int R1, int R2, int VL = 1, bool SLOTRED = false>
+// ZS > 0: retire into the per-warp slab of ZS cell layers (dynamic shared memory after the NW records).
+template <int N, int ZS> struct SlabCfg {
+    static constexpr int SX = 8 + N, SY = 8 + N, SZ = ZS + N;    // nodes per direction (N+1 per quiet line)
+    static constexpr int SN = SX * SY * SZ;                      // doubles per component
+};
+template <int N, int NW, int MINB, int R0, int R1, int R2, int VL = 1, bool SLOTRED = false, int ZS = 0>
 __global__ void __launch_bounds__(NW * 32, MINB)
 deposit_quiet_kernel(SoaView P, long np, int chunks_per_warp, J3 Jp, DepositGeom dg, KeyBase kbp,
                      int* __restrict__ list, int* __restrict__ list_count) {
     // role views of the physical arrays / geometry
     const FabView& Jx = Jp.v[R0]; const FabView& Jy = Jp.v[R1]; const FabView& Jz = Jp.v[R2];
-    const long stX = fab_stride(Jx, R0), stY = fab_stride(Jy, R1), stZ = fab_stride(Jz, R2);
     const int kbb[3] = {kbp.b0, kbp.b1, kbp.b2};
     const KeyBase kb = {kbb[R0], kbb[R1], kbb[R2]};
     using T = QuietCfg<N, VL>;
     constexpr int QS = T::QS, QL = T::QL, NG = T::NG, QP = T::QP, NF = T::NF, CHP = T::CHP;
+    constexpr bool SLAB = ZS > 0;
+    static_assert(!SLAB || (VL == 1 && !SLOTRED), "the slab takes one sender lane per line");
+    using SC = SlabCfg<N, (SLAB ? ZS : 1)>;
+    constexpr int SX = SC::SX, SY = SC::SY, SN = SC::SN;
     PIC_DYNAMIC_SMEM(double2, smem2);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     double2* rec = smem2 + (size_t)warp * NF * CHP;
+    double* slab = reinterpret_cast<double*>(smem2 + (size_t)NW * NF * CHP) + (size_t)warp * 3 * SN;
+    // strides of the window's lines: along its own role in the slab or in J, and along role X for Jy / Jz
+    const long stX = SLAB ? 1 : fab_stride(Jx, R0), stY = SLAB ? SX : fab_stride(Jy, R1);
+    const long stZ = SLAB ? (long)SX * SY : fab_stride(Jz, R2);
+    const long xY = SLAB ? 1 : fab_stride(Jy, R0), xZ = SLAB ? 1 : fab_stride(Jz, R0);
 
     const long nchunks = (np + DR_CH - 1) / DR_CH;
     const long wg = (long)blockIdx.x * NW + warp;
@@ -153,84 +190,146 @@ deposit_quiet_kernel(SoaView P, long np, int chunks_per_warp, J3 Jp, DepositGeom
         q[R0] = ix; q[R1] = iy; q[R2] = iz;
         return F.p + F.off(q[0], q[1], q[2]);
     };
+    // The slab holds the nodes (bx.., by.., bz..) of role component c at slab[c*SN + (z*SY + y)*SX + x]; it
+    // takes the anchors gx+1 - bx in [0, 8), gy+1 - by in [0, 8), gz+1 - bz in [0, ZS).  No base yet: bx huge.
+    int bx = 1 << 28, by = 0, bz = 0;
+    auto slab_at = [&](int c, int ix, int iy, int iz) -> double* {       // role indices -> slab node
+        return slab + c * SN + ((iz - bz) * SY + (iy - by)) * SX + (ix - bx);
+    };
+    auto covers = [&](int k) -> bool {
+        const int gx = (k & 1023) + kb.b0, gy = ((k >> 10) & 1023) + kb.b1, gz = (k >> 20) + kb.b2;
+        return (unsigned)(gx + 1 - bx) < 8u && (unsigned)(gy + 1 - by) < 8u && (unsigned)(gz + 1 - bz) < (unsigned)ZS;
+    };
+    // add the slab to J (red.global along x rows, zeros skipped), zero it and base it at anchor k: x and y at
+    // the supercell of k's cell (gx + 2 for order 3), z at k's own layer
+    auto rebase = [&](int k) {
+        if (bx != (1 << 28)) {
+            DR_COUNT(rebases, lane == 0);
+#pragma unroll 1
+            for (int c = 0; c < 3; ++c) {
+                const FabView& F = c == 0 ? Jx : (c == 1 ? Jy : Jz);
+#pragma unroll 1
+                for (int e = lane; e < SN; e += 32) {
+                    const double v = slab[c * SN + e];
+                    if (v != 0.0) { atomicAdd(at(F, bx + e % SX, by + (e / SX) % SY, bz + e / (SX * SY)), v); DR_COUNT(red_slab, 1); }
+                }
+            }
+            __syncwarp();                          // every node read before any lane zeroes it
+        }
+        if (k >= 0) {
+            const int gx = (k & 1023) + kb.b0, gy = ((k >> 10) & 1023) + kb.b1, gz = (k >> 20) + kb.b2;
+            bx = ((gx + 2) & ~7) - 1; by = ((gy + 2) & ~7) - 1; bz = gz + 1;
+#pragma unroll 1
+            for (int e = lane; e < 3 * SN; e += 32) slab[e] = 0.0;
+        }
+        __syncwarp();
+    };
     auto set_anchor = [&](int k) {
         const int ax = (k & 1023), gx = ax + kb.b0, gy = ((k >> 10) & 1023) + kb.b1, gz = (k >> 20) + kb.b2;
         ur = ring(ax);
+        DR_COUNT(cells, lane == 0);
 #pragma unroll
         for (int m = 0; m < VL; ++m) {
             const int qv = qv0 + m;
-            px[m] = at(Jx, gx + 1, gy + 1 + qu, gz + 1 + qv);
-            py[m] = at(Jy, gx + 1 + ur, gy + 1, gz + 1 + qv);
-            pz[m] = at(Jz, gx + 1 + ur, gy + 1 + qv, gz + 1);
+            if constexpr (SLAB) {
+                px[m] = slab_at(0, gx + 1, gy + 1 + qu, gz + 1 + qv);
+                py[m] = slab_at(1, gx + 1 + ur, gy + 1, gz + 1 + qv);
+                pz[m] = slab_at(2, gx + 1 + ur, gy + 1 + qv, gz + 1);
+            } else {
+                px[m] = at(Jx, gx + 1, gy + 1 + qu, gz + 1 + qv);
+                py[m] = at(Jy, gx + 1 + ur, gy + 1, gz + 1 + qv);
+                pz[m] = at(Jz, gx + 1 + ur, gy + 1 + qv, gz + 1);
+            }
         }
+    };
+    auto put = [&](double* p, double v) {         // retire one partial sum
+        if constexpr (SLAB) *p += v;
+        else { atomicAdd(p, v); DR_COUNT(red_retire, 1); }
     };
     // the anchor advances one cell along x: only the plane x = gx+1 leaves the window
     auto slide = [&]() {
         const bool leaving = (ur == 0);
+        DR_COUNT(slides, lane == 0);
+        DR_COUNT(cells, lane == 0);
 #pragma unroll
         for (int m = 0; m < VL; ++m) {
             const double vx = fold(acc[m][0][0]);
-            if (sender) atomicAdd(px[m], vx);
+            if (sender) put(px[m], vx);
 #pragma unroll
             for (int i = 0; i + 1 < QP; ++i) acc[m][0][i] = acc[m][0][i + 1];
             acc[m][0][QP - 1] = 0.0;
 #pragma unroll
             for (int i = 0; i < QP; ++i) {
                 const double vy = fold(acc[m][1][i]), vz = fold(acc[m][2][i]);
-                if (sender && leaving) { atomicAdd(py[m] + i * stY, vy); atomicAdd(pz[m] + i * stZ, vz); }
+                if (sender && leaving) { put(py[m] + i * stY, vy); put(pz[m] + i * stZ, vz); }
                 if (leaving) { acc[m][1][i] = 0.0; acc[m][2][i] = 0.0; }
             }
             px[m] += stX;                               // next X plane
-            if (leaving) { py[m] += QS * fab_stride(Jy, R0); pz[m] += QS * fab_stride(Jz, R0); }   // now owns X = gx + 1 + QS
+            if (leaving) { py[m] += QS * xY; pz[m] += QS * xZ; }   // now owns X = gx + 1 + QS
         }
         if (leaving) ur = QS - 1;
         else ur -= 1;                                   // same absolute x, one slot lower
+        if constexpr (SLAB) __syncwarp();
     };
     auto flush_all = [&]() {                        // the anchor jumps: retire the whole window
+        DR_COUNT(jumps, lane == 0);
 #pragma unroll
         for (int m = 0; m < VL; ++m)
 #pragma unroll
             for (int i = 0; i < QP; ++i) {
                 const double vx = fold(acc[m][0][i]), vy = fold(acc[m][1][i]), vz = fold(acc[m][2][i]);
-                if (sender) { atomicAdd(px[m] + i * stX, vx); atomicAdd(py[m] + i * stY, vy); atomicAdd(pz[m] + i * stZ, vz); }
+                if (sender) { put(px[m] + i * stX, vx); put(py[m] + i * stY, vy); put(pz[m] + i * stZ, vz); }
                 acc[m][0][i] = 0.0; acc[m][1][i] = 0.0; acc[m][2][i] = 0.0;
             }
+        if constexpr (SLAB) __syncwarp();
     };
 
-    // one particle (record column pq) of anchor k, deposited without the register window
+    // one particle (record column pq) of anchor k, deposited without the register window: into the slab when it
+    // covers k, else straight to J
     auto deposit_lone = [&](int k, int pq) {
-        if (lane >= QL) return;
-        const int ax = (k & 1023), gx = ax + kb.b0, gy = ((k >> 10) & 1023) + kb.b1, gz = (k >> 20) + kb.b2;
-        const int us = ring(ax);
-        const double2 sx = rec[(T::F_SX + us) * CHP + pq];
-        const double2 sy = rec[(T::F_SY + qu) * CHP + pq];
+        const bool in_slab = SLAB && covers(k);
+        DR_COUNT(lones, lane == 0);
+        DR_COUNT(lones_outside, lane == 0 && !in_slab);
+        if (lane < QL) {
+            const int ax = (k & 1023), gx = ax + kb.b0, gy = ((k >> 10) & 1023) + kb.b1, gz = (k >> 20) + kb.b2;
+            const int us = ring(ax);
+            const double2 sx = rec[(T::F_SX + us) * CHP + pq];
+            const double2 sy = rec[(T::F_SY + qu) * CHP + pq];
+            const long lX = in_slab ? 1 : fab_stride(Jx, R0), lY = in_slab ? SX : fab_stride(Jy, R1);
+            const long lZ = in_slab ? (long)SX * SY : fab_stride(Jz, R2);
 #pragma unroll
-        for (int mv = 0; mv < VL; ++mv) {
-            const int qv = qv0 + mv;
-            double* qx = at(Jx, gx + 1, gy + 1 + qu, gz + 1 + qv);
-            double* qy = at(Jy, gx + 1 + us, gy + 1, gz + 1 + qv);
-            double* qz = at(Jz, gx + 1 + us, gy + 1 + qv, gz + 1);
-            const double2 aby = rec[(T::F_ABY + qv) * CHP + pq];
-            const double2 abz = rec[(T::F_ABZ + qv) * CHP + pq];
-            const double wx = sy.x * abz.x + sy.y * abz.y;
-            const double wy = sx.x * abz.x + sx.y * abz.y;
-            const double wz = sx.x * aby.x + sx.y * aby.y;
+            for (int mv = 0; mv < VL; ++mv) {
+                const int qv = qv0 + mv;
+                double* qx = in_slab ? slab_at(0, gx + 1, gy + 1 + qu, gz + 1 + qv) : at(Jx, gx + 1, gy + 1 + qu, gz + 1 + qv);
+                double* qy = in_slab ? slab_at(1, gx + 1 + us, gy + 1, gz + 1 + qv) : at(Jy, gx + 1 + us, gy + 1, gz + 1 + qv);
+                double* qz = in_slab ? slab_at(2, gx + 1 + us, gy + 1 + qv, gz + 1) : at(Jz, gx + 1 + us, gy + 1 + qv, gz + 1);
+                auto add = [&](double* q, double v) {
+                    if (in_slab) *q += v;
+                    else { atomicAdd(q, v); DR_COUNT(red_lone, 1); }
+                };
+                const double2 aby = rec[(T::F_ABY + qv) * CHP + pq];
+                const double2 abz = rec[(T::F_ABZ + qv) * CHP + pq];
+                const double wx = sy.x * abz.x + sy.y * abz.y;
+                const double wy = sx.x * abz.x + sx.y * abz.y;
+                const double wz = sx.x * aby.x + sx.y * aby.y;
 #pragma unroll
-            for (int m = 0; m < T::NCDS; ++m) {
-                const double2 c2 = rec[(T::F_CDS + m) * CHP + pq];
+                for (int m = 0; m < T::NCDS; ++m) {
+                    const double2 c2 = rec[(T::F_CDS + m) * CHP + pq];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int e = 2 * m + h;                 // entry e = component (e / QP), prefix index (e % QP)
-                    if (e < 3 * QP) {
-                        const double cv = h ? c2.y : c2.x;
-                        const int c = e / QP, i = e % QP;
-                        if (c == 0) atomicAdd(qx + i * stX, cv * wx);
-                        else if (c == 1) atomicAdd(qy + i * stY, cv * wy);
-                        else atomicAdd(qz + i * stZ, cv * wz);
+                    for (int h = 0; h < 2; ++h) {
+                        const int e = 2 * m + h;                 // entry e = component (e / QP), prefix index (e % QP)
+                        if (e < 3 * QP) {
+                            const double cv = h ? c2.y : c2.x;
+                            const int c = e / QP, i = e % QP;
+                            if (c == 0) add(qx + i * lX, cv * wx);
+                            else if (c == 1) add(qy + i * lY, cv * wy);
+                            else add(qz + i * lZ, cv * wz);
+                        }
                     }
                 }
             }
         }
+        if constexpr (SLAB) __syncwarp();
     };
 
     // software prefetch: chunk ch+1 is requested before chunk ch is processed
@@ -303,6 +402,9 @@ deposit_quiet_kernel(SoaView P, long np, int chunks_per_warp, J3 Jp, DepositGeom
                 basei = __shfl_sync(FULL, basei, 0);
                 if (moved) list[basei + __popc(mm & ((1u << lane) - 1u))] = (int)(base + lane);
             }
+            DR_COUNT(chunks, lane == 0);
+            DR_COUNT(particles, lane < nval);
+            DR_COUNT(movers, moved);
         }
         __syncwarp();
         // ---------------- phase 2: lane = stencil lines ----------------
@@ -325,9 +427,15 @@ deposit_quiet_kernel(SoaView P, long np, int chunks_per_warp, J3 Jp, DepositGeom
                 const int k = __shfl_sync(FULL, key, start);
                 if ((lones >> start) & 1u) { deposit_lone(k, start); continue; }
                 if (k < 0) continue;
+                DR_COUNT(runs, lane == 0);
                 if (k != cur) {
-                    if (cur >= 0 && k == cur + 1) slide();
-                    else { if (cur >= 0) flush_all(); set_anchor(k); }
+                    const bool inside = !SLAB || covers(k);
+                    if (cur >= 0 && k == cur + 1 && inside) slide();
+                    else {
+                        if (cur >= 0) flush_all();
+                        if (!inside) rebase(k);
+                        set_anchor(k);
+                    }
                     cur = k;
                 }
                 auto accumulate = [&](int pq) {
@@ -362,6 +470,7 @@ deposit_quiet_kernel(SoaView P, long np, int chunks_per_warp, J3 Jp, DepositGeom
         __syncwarp();
     }
     if (cur >= 0) flush_all();
+    if constexpr (SLAB) rebase(-1);
 }
 
 // ================================================================================================
@@ -377,6 +486,8 @@ template <int N> struct GeneralCfg {
     static constexpr int F_AY = 4 * S, F_BY = 5 * S, F_AZ = 6 * S, F_BZ = 7 * S;
     static constexpr int F_CDS = 8 * S;
     static constexpr int NF = 8 * S + 3 * PN;
+    static constexpr int NJX = S * S * PN;          // Jx of one stencil, staged x-fastest before it goes to J
+    static constexpr int WARP_DOUBLES = NF * DR_CHP + NJX;   // shared memory per warp
 };
 
 template <int N, int NW>
@@ -387,7 +498,8 @@ deposit_general_kernel(SoaView P, const int* __restrict__ list, const int* __res
     constexpr int S = T::S, PN = T::PN, NB = T::NB, NF = T::NF, CHP = DR_CHP;
     PIC_DYNAMIC_SMEM(double, smem);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double* rec = smem + (size_t)warp * NF * CHP;
+    double* rec = smem + (size_t)warp * T::WARP_DOUBLES;
+    double* xs = rec + NF * CHP;
     const int count = *list_count;
     const int nchunks = (count + DR_CH - 1) / DR_CH;
     // lane (a, bh) owns lines (a, b), b = bh + nb*BH:  Jx (j=a,k=b), Jy (i=a,k=b), Jz (i=a,j=b)
@@ -401,26 +513,38 @@ deposit_general_kernel(SoaView P, const int* __restrict__ list, const int* __res
 #pragma unroll
             for (int i = 0; i < PN; ++i) acc[nb][c][i] = 0.0;
 
+    // Called by the whole warp (k is warp-uniform).  Jy and Jz go to J from the lines: the lanes of one
+    // reduction differ in x by a, so S of them share a row.  The Jx lines run along x themselves, so one
+    // reduction would touch 18 different rows; Jx is staged in xs instead and sent x-fastest, a warp
+    // instruction then covering rows of PN consecutive nodes.
     auto flush = [&](int k) {
-        if (k < 0 || !active) return;
+        if (k < 0) return;
         const int gx = (k & 1023) + kb.b0, gy = ((k >> 10) & 1023) + kb.b1, gz = (k >> 20) + kb.b2;
+        if (active) {
 #pragma unroll
-        for (int nb = 0; nb < NB; ++nb) {
-            const int b = bh + nb * T::BH;
-            if (b < S) {
-                double* px = &Jx(gx, gy + a, gz + b);
-                double* py = &Jy(gx + a, gy, gz + b);
-                double* pz = &Jz(gx + a, gy + b, gz);
+            for (int nb = 0; nb < NB; ++nb) {
+                const int b = bh + nb * T::BH;
+                if (b < S) {
+                    double* py = &Jy(gx + a, gy, gz + b);
+                    double* pz = &Jz(gx + a, gy + b, gz);
 #pragma unroll
-                for (int i = 0; i < PN; ++i) {
-                    const double vx = acc[nb][0][i], vy = acc[nb][1][i], vz = acc[nb][2][i];
-                    if (vx != 0.0) atomicAdd(px + i, vx);
-                    if (vy != 0.0) atomicAdd(py + i * Jy.sj, vy);
-                    if (vz != 0.0) atomicAdd(pz + i * Jz.sk, vz);
-                    acc[nb][0][i] = 0.0; acc[nb][1][i] = 0.0; acc[nb][2][i] = 0.0;
+                    for (int i = 0; i < PN; ++i) {
+                        const double vy = acc[nb][1][i], vz = acc[nb][2][i];
+                        xs[(b * S + a) * PN + i] = acc[nb][0][i];        // Jx(gx + i, gy + a, gz + b)
+                        if (vy != 0.0) atomicAdd(py + i * Jy.sj, vy);
+                        if (vz != 0.0) atomicAdd(pz + i * Jz.sk, vz);
+                        acc[nb][0][i] = 0.0; acc[nb][1][i] = 0.0; acc[nb][2][i] = 0.0;
+                    }
                 }
             }
         }
+        __syncwarp();
+#pragma unroll 1
+        for (int e = lane; e < T::NJX; e += 32) {
+            const double v = xs[e];
+            if (v != 0.0) atomicAdd(&Jx(gx + e % PN, gy + (e / PN) % S, gz + e / (PN * S)), v);
+        }
+        __syncwarp();                                  // xs read by every lane before the next flush writes it
     };
 
     for (int ch = blockIdx.x * NW + warp; ch < nchunks; ch += gridDim.x * NW) {
@@ -545,14 +669,22 @@ static int launch_runs(SoaView P, long np, const pic_fab J[3], const DepositGeom
     const bool two = !four && (g_runs_variant & 1) && VL2 == 2, slotred = (g_runs_variant & 2) != 0;
     constexpr int VL4 = (N == 3) ? 4 : 1;
     using TQ4 = QuietCfg<N, VL4>;
+    // J slab: 2 cell layers, 4 warps x 2 CTAs per SM (104 KB of shared memory per CTA, 154 registers, no spills;
+    // 3 warps x 3 CTAs with one layer and 2 warps x 4 CTAs measured the same)
+    const bool slab = !four && !two && !slotred && (g_runs_variant & 8);
+    using TS2 = SlabCfg<N, 2>;
     auto kq = four ? (slotred ? deposit_quiet_kernel<N, NWQ, 3, 0, 1, 2, VL4, true> : deposit_quiet_kernel<N, NWQ, 3, 0, 1, 2, VL4, false>)
             : two ? (slotred ? deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, VL2, true> : deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, VL2, false>)
-                  : (slotred ? deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, true> : deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, false>);
+            : slotred ? deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, true>
+            : !slab ? deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, false>
+            : deposit_quiet_kernel<N, 4, 2, 0, 1, 2, 1, false, 2>;
+    const int nwq = 4;
     auto kg = deposit_general_kernel<N, NWG>;
-    const size_t smem_q = (size_t)NWQ * TQ::NF * (four ? TQ4::CHP : two ? TQ2::CHP : TQ::CHP) * sizeof(double2);
-    const size_t smem_g = (size_t)NWG * TG::NF * DR_CHP * sizeof(double);
-    static bool attr_done[8] = {false, false, false, false, false, false, false, false};
-    const int vidx = (two ? 1 : 0) + (slotred ? 2 : 0) + (four ? 4 : 0);
+    const size_t smem_q = (size_t)nwq * TQ::NF * (four ? TQ4::CHP : two ? TQ2::CHP : TQ::CHP) * sizeof(double2) +
+                          (slab ? (size_t)nwq * 3 * TS2::SN * sizeof(double) : 0);
+    const size_t smem_g = (size_t)NWG * TG::WARP_DOUBLES * sizeof(double);
+    static bool attr_done[16] = {false};
+    const int vidx = (two ? 1 : 0) + (slotred ? 2 : 0) + (four ? 4 : 0) + (slab ? 8 : 0);
     if (!attr_done[vidx]) {
         cudaFuncSetAttribute(kq, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_q);
         cudaFuncSetAttribute(kg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_g);
@@ -561,9 +693,9 @@ static int launch_runs(SoaView P, long np, const pic_fab J[3], const DepositGeom
     const long nchunks = (np + DR_CH - 1) / DR_CH;
     const int cpw = 16;   // 512 consecutive particles per warp: long runs, few boundaries
     const long nwarps = (nchunks + cpw - 1) / cpw;
-    const unsigned grid_q = (unsigned)((nwarps + NWQ - 1) / NWQ);
+    const unsigned grid_q = (unsigned)((nwarps + nwq - 1) / nwq);
     J3 j3; j3.v[0] = make_view(J[0]); j3.v[1] = make_view(J[1]); j3.v[2] = make_view(J[2]);
-    kq<<<grid_q, NWQ * 32, smem_q, s>>>(P, np, cpw, j3, dg, kb, list, list_count);
+    kq<<<grid_q, nwq * 32, smem_q, s>>>(P, np, cpw, j3, dg, kb, list, list_count);
     kg<<<NUM_SMS * 3, NWG * 32, smem_g, s>>>(P, list, list_count, make_view(J[0]), make_view(J[1]), make_view(J[2]), dg, kb);
     count_launch(2);
     cudaFreeAsync(scratch, s);
@@ -580,22 +712,27 @@ static int launch_runs(SoaView P, long np, const pic_fab J[3], const DepositGeom
     const bool two = !four && (g_runs_variant & 1) && VL2 == 2, slotred = (g_runs_variant & 2) != 0;
     constexpr int VL4 = (N == 3) ? 4 : 1;
     using TQ4 = QuietCfg<N, VL4>;
-    const size_t smem_q = (size_t)NWQ * TQ::NF * (four ? TQ4::CHP : two ? TQ2::CHP : TQ::CHP) * sizeof(double2);
-    const size_t smem_g = (size_t)NWG * TG::NF * DR_CHP * sizeof(double);
+    const bool slab = !four && !two && !slotred && (g_runs_variant & 8);
+    using TS2 = SlabCfg<N, 2>;
+    const int nwq = 4;
+    const size_t smem_q = (size_t)nwq * TQ::NF * (four ? TQ4::CHP : two ? TQ2::CHP : TQ::CHP) * sizeof(double2) +
+                          (slab ? (size_t)nwq * 3 * TS2::SN * sizeof(double) : 0);
+    const size_t smem_g = (size_t)NWG * TG::WARP_DOUBLES * sizeof(double);
     const long nchunks = (np + DR_CH - 1) / DR_CH;
     const int cpw = 16;
     const long nwarps = (nchunks + cpw - 1) / cpw;
-    const unsigned grid_q = (unsigned)((nwarps + NWQ - 1) / NWQ);
+    const unsigned grid_q = (unsigned)((nwarps + nwq - 1) / nwq);
     J3 j3; j3.v[0] = make_view(J[0]); j3.v[1] = make_view(J[1]); j3.v[2] = make_view(J[2]);
     const FabView v0 = make_view(J[0]), v1 = make_view(J[1]), v2 = make_view(J[2]);
     (void)s;
-    ::simt::launch(dim3(grid_q), dim3(NWQ * 32), smem_q, [&] {
+    ::simt::launch(dim3(grid_q), dim3(nwq * 32), smem_q, [&] {
         if (four && slotred) deposit_quiet_kernel<N, NWQ, 3, 0, 1, 2, VL4, true>(P, np, cpw, j3, dg, kb, list, list_count);
         else if (four) deposit_quiet_kernel<N, NWQ, 3, 0, 1, 2, VL4, false>(P, np, cpw, j3, dg, kb, list, list_count);
         else if (two && slotred) deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, VL2, true>(P, np, cpw, j3, dg, kb, list, list_count);
         else if (two) deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, VL2, false>(P, np, cpw, j3, dg, kb, list, list_count);
         else if (slotred) deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, true>(P, np, cpw, j3, dg, kb, list, list_count);
-        else deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, false>(P, np, cpw, j3, dg, kb, list, list_count);
+        else if (!slab) deposit_quiet_kernel<N, NWQ, MINB, 0, 1, 2, 1, false>(P, np, cpw, j3, dg, kb, list, list_count);
+        else deposit_quiet_kernel<N, 4, 2, 0, 1, 2, 1, false, 2>(P, np, cpw, j3, dg, kb, list, list_count);
     });
     ::simt::launch(dim3(4), dim3(NWG * 32), smem_g,
                    [&] { deposit_general_kernel<N, NWG>(P, list, list_count, v0, v1, v2, dg, kb); });
@@ -616,7 +753,7 @@ static int launch_general(SoaView P, const int* list, const int* list_count, con
     kb.b0 = min(J[0].lo[0], min(J[1].lo[0], J[2].lo[0])) - 1;
     kb.b1 = min(J[0].lo[1], min(J[1].lo[1], J[2].lo[1])) - 1;
     kb.b2 = min(J[0].lo[2], min(J[1].lo[2], J[2].lo[2])) - 1;
-    const size_t smem_g = (size_t)NWG * TG::NF * DR_CHP * sizeof(double);
+    const size_t smem_g = (size_t)NWG * TG::WARP_DOUBLES * sizeof(double);
     auto kg = deposit_general_kernel<N, NWG>;
 #ifndef PIC_SIMT_HOST
     static bool attr_done = false;
