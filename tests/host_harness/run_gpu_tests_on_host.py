@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""TEST INFRASTRUCTURE -- runs the `-m gpu` test functions (tests/test_gpu_parity.py, tests/test_gpu_zz_lwfa.py)
+"""TEST INFRASTRUCTURE -- runs the `-m gpu` test functions (tests/test_gpu_parity.py, tests/test_gpu_particle_sets.py,
+tests/test_gpu_zz_lwfa.py)
 against the HOST build of the library (harness.host_library: every csrc file compiled by g++ against the SIMT emulator),
 for a container without a GPU:
 
@@ -63,6 +64,7 @@ class _TorchOnHost:
 
 
 import test_gpu_parity as TP  # noqa: E402
+import test_gpu_particle_sets as TS  # noqa: E402
 import test_gpu_zz_lwfa as TL  # noqa: E402
 from oracle import oracle as orc  # noqa: E402
 
@@ -97,7 +99,7 @@ def main():
     minus = [w[1:] for w in sys.argv[1:] if w.startswith("-")]
     golden = json.load(open(os.path.join(TESTS, "golden", "warpx_checksums.json")))
     npass = nfail = 0
-    for mod in (TP, TL):
+    for mod in (TP, TS, TL):
         for name, fn in sorted(vars(mod).items()):
             if not name.startswith("test_") or not inspect.isfunction(fn) or fn.__module__ != mod.__name__:
                 continue

@@ -18,7 +18,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
 
+import particle_sets as ps  # noqa: E402
 from helpers import lower_corner, rel_linf  # noqa: E402
+from particle_sets import steady_state  # noqa: E402
 from warpx_b200 import abi, workloads  # noqa: E402
 
 COUNTERS = ("chunks", "particles", "movers", "runs", "slides", "jumps", "lones", "lones_outside", "rebases", "cells",
@@ -49,29 +51,6 @@ def counting_simt():
     return L
 
 
-def steady_state(n=(16, 16, 8), u_th=0.05, steps=24, after_sort=3, nox=3):
-    """Particles of a thermal plasma after `steps` oracle steps, sorted into the engine's bin order (8^3 supercells,
-    cells x-fastest inside), then `after_sort` more steps; with the oracle run that produced them."""
-    from oracle import oracle
-    dx = 40.0e-6 / 256
-    lx = tuple(dx * v for v in n)
-    wl = workloads.uniform_plasma_3d(n_cell=n, ppc=(2, 2, 2), u_th=u_th, lx=lx)
-    s = wl["species"][0]
-    sim = oracle.OracleSim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=nox)
-    sim.add_species(s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
-    sim.evolve(steps)
-    p = sim.particles(0)
-    cell = [np.clip(np.floor((p[k] - wl["prob_lo"][d]) / dx).astype(np.int64), 0, n[d] - 1) for d, k in enumerate("xyz")]
-    nt = [(v + 7) // 8 for v in n]
-    tile = cell[0] // 8 + nt[0] * (cell[1] // 8 + nt[1] * (cell[2] // 8))
-    key = tile * 512 + cell[0] % 8 + 8 * (cell[1] % 8 + 8 * (cell[2] % 8))
-    order = np.argsort(key, kind="stable")
-    sim2 = oracle.OracleSim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=nox)
-    sim2.add_species(s["q"], s["m"], *[p[k][order] for k in ("x", "y", "z", "w", "ux", "uy", "uz")])
-    sim2.evolve(after_sort)
-    return wl, sim2.dt, sim2.particles(0)
-
-
 def deposit_both(L, wl, dt, p, variant, nox=3):
     from oracle import oracle as orc
     n = wl["n_cell"]
@@ -97,7 +76,8 @@ def deposit_both(L, wl, dt, p, variant, nox=3):
 
 @pytest.fixture(scope="module")
 def state():
-    return counting_simt(), steady_state()
+    wl, dt, p, _ = steady_state()
+    return counting_simt(), (wl, dt, p)
 
 
 @pytest.mark.parametrize("variant", [0, VARIANT_SLAB])
@@ -115,12 +95,31 @@ def test_run_kernel_matches_oracle_in_steady_state(orc, state, variant):
         assert cnt["rebases"] == 0 and cnt["red_slab"] == 0 and cnt["red_retire"] > 0
 
 
+@pytest.mark.parametrize("variant", [0, VARIANT_SLAB])
+@pytest.mark.parametrize("name", ["steady", "poisson", "crowded_movers"])
+def test_run_kernel_matches_oracle_on_particle_sets(orc, state, name, variant):
+    """The sets of tests/particle_sets.py (log-uniform weights; Poisson counts with runs longer than a warp's span;
+    a supercell of diagonal movers) through both retire paths, order 3."""
+    L = state[0]
+    s = ps.get(name)
+    wl = dict(n_cell=s.n, prob_lo=s.prob_lo, prob_hi=s.prob_hi, species=[dict(q=s.q)])
+    J, K, cnt = deposit_both(L, wl, s.dt, s.p, variant)
+    for c in range(3):
+        assert rel_linf(K[c].a, J[c].a) <= 1e-13, "j" + "xyz"[c]
+    # the kernel classifies the particles as the numpy restatement of tests/test_particle_sets.py does
+    want = ps.quiet_kernel_events(s, 3, (5, 5, 5))
+    assert cnt["movers"] == want["movers"] and cnt["lones"] == want["lones"], (cnt, want)
+    assert cnt["runs"] > 0 and (name != "steady" or cnt["lones"] > 0)
+    if variant == VARIANT_SLAB:
+        assert cnt["red_slab"] > 0 and cnt["red_retire"] == 0
+
+
 def main():
     """Counts per deposited step over one sort interval (1..4 steps after the sort), both retire paths."""
     L = counting_simt()
     tot = {v: dict.fromkeys(COUNTERS, 0) for v in (0, VARIANT_SLAB)}
     for k in range(4):
-        wl, dt, p = steady_state(n=(32, 32, 16), u_th=0.01, steps=60, after_sort=k + 1)
+        wl, dt, p, _ = steady_state(n=(32, 32, 16), u_th=0.01, steps=60, after_sort=k + 1)
         for v in tot:
             _, _, cnt = deposit_both(L, wl, dt, p, v)
             for f in COUNTERS:

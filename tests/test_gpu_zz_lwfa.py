@@ -15,6 +15,7 @@ import pytest
 from helpers import rel_linf
 from helpers import lower_corner, random_fields
 from test_gpu_parity import Dev, _particles, _run_both, _match_particles, _sorted_device_species, box  # noqa: F401
+from test_gpu_parity import add_background, check_on_background
 from test_oracle import check_particle_boundaries, check_pec_particle, make_lwfa_oracle
 from warpx_b200 import abi, workloads
 
@@ -687,13 +688,17 @@ def test_charge_deposition_matches_oracle(orc, dev, nox):
 
 
 # ---------------------------------------------------------------------------------------------
-# Experimental variants of the register-run deposition (pic_set_deposit_mode 2, 3, 4; DESIGN.md section 8):
-# same parity bar as the default kernel.  (Checked under the SIMT emulator on the host: test_simt_host.py.)
+# Variants of the cell-sorted deposition (pic_set_deposit_mode; DESIGN.md sections 3.3 and 8): same parity bar as the
+# default kernel, J starting from a random background.  (Checked under the SIMT emulator on the host: test_simt_host.py;
+# on adversarial particle sets: test_gpu_particle_sets.py.)
 # ---------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("mode", [2, 3, 4, 5, 6, 7, 8, 9, 10, 11])
+@pytest.mark.parametrize("mode", [abi.PIC_DEPOSIT_RUNS2, abi.PIC_DEPOSIT_RUNS_SLOTRED, abi.PIC_DEPOSIT_RUNS2_SLOTRED,
+                                  abi.PIC_DEPOSIT_RUNS4, abi.PIC_DEPOSIT_RUNS4_SLOTRED, abi.PIC_DEPOSIT_CELLS,
+                                  abi.PIC_DEPOSIT_CELLS2, abi.PIC_DEPOSIT_CELLS2_WIDE, abi.PIC_DEPOSIT_CELLS3,
+                                  abi.PIC_DEPOSIT_CELLS3_WIDE, abi.PIC_DEPOSIT_RUNS_SLAB])
 @pytest.mark.parametrize("nox,kind", [(3, "sorted"), (3, "drifted"), (1, "sorted"), (2, "sorted"), (3, "relativistic")])
 def test_deposit_variants_match_oracle(orc, dev, mode, nox, kind):
-    if mode in (5, 6) and nox != 3:
+    if mode in (abi.PIC_DEPOSIT_RUNS4, abi.PIC_DEPOSIT_RUNS4_SLOTRED) and nox != 3:
         pytest.skip("four lines per lane: order 3 only")
     L = orc.lib()
     n, lx = (20, 16, 12), 1e-5
@@ -714,6 +719,9 @@ def test_deposit_variants_match_oracle(orc, dev, mode, nox, kind):
         buf[0:3] += dev.t.tensor([[0.8 * dx[0]], [-0.9 * dx[1]], [0.6 * dx[2]]], device="cuda")
     host = buf.cpu().numpy()
     P = orc.HostParticles(**{k: host[i] for i, k in enumerate(orc.HostParticles.NAMES)})
+    L.orc_deposit_esirkepov(C.byref(P.soa), 0, P.np, orc.fab_array(J), abi.dbl3(dinv), abi.dbl3(xyzmin),
+                            abi.int3(lo), sp["q"], dt, -0.5 * dt, nox)
+    B = add_background(dev, J, tens, mode)
     dev.L.pic_set_deposit_mode(mode)
     try:
         dev.ok(dev.L.pic_deposit_esirkepov(C.byref(Pd), 0, P.np, (abi.pic_fab * 3)(*arr), abi.dbl3(dinv), abi.dbl3(xyzmin),
@@ -721,10 +729,7 @@ def test_deposit_variants_match_oracle(orc, dev, mode, nox, kind):
         dev.sync()
     finally:
         dev.L.pic_set_deposit_mode(0)
-    L.orc_deposit_esirkepov(C.byref(P.soa), 0, P.np, orc.fab_array(J), abi.dbl3(dinv), abi.dbl3(xyzmin),
-                            abi.int3(lo), sp["q"], dt, -0.5 * dt, nox)
-    for c in range(3):
-        assert rel_linf(tens[c].cpu().numpy(), J[c].a) <= 1e-12, "j" + "xyz"[c]
+    check_on_background([t.cpu().numpy() for t in tens], [f.a for f in J], B)
 
 
 @pytest.mark.parametrize("mode", [1, 2, 3])

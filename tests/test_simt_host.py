@@ -10,7 +10,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import particle_sets as ps
 from helpers import lower_corner, rel_linf
+from particle_sets import host_bins
 from warpx_b200 import abi, workloads
 
 
@@ -62,22 +64,6 @@ def test_deposit_runs_kernels_under_simt_emulation(orc, simt, variant, nox, u_th
 # ---------------------------------------------------------------------------------------------------------
 # the supercell gather + push kernels of warpx_b200/csrc/gather_push_tile.cu under the same emulator
 # ---------------------------------------------------------------------------------------------------------
-def host_bins(x, y, z, prob_lo, dx, n, tile):
-    """pic_bins on the host: the supercell-major bin of every particle (bins.cuh::bin_of_cell), a stable sort by bin
-    and the cell_start table -- what the device counting sort produces."""
-    n, tile = np.asarray(n), np.asarray(tile)
-    nt = (n + tile - 1) // tile
-    cell = [np.clip(np.floor((v - prob_lo[d]) / dx[d]).astype(np.int64), 0, n[d] - 1) for d, v in enumerate((x, y, z))]
-    t = [cell[d] // tile[d] for d in range(3)]
-    li = [cell[d] - t[d] * tile[d] for d in range(3)]
-    tid = t[0] + nt[0] * (t[1] + nt[1] * t[2])
-    b = tid * int(np.prod(tile)) + li[0] + tile[0] * (li[1] + tile[1] * li[2])
-    order = np.argsort(b, kind="stable")
-    nbins = int(np.prod(nt) * np.prod(tile))
-    cell_start = np.searchsorted(b[order], np.arange(nbins + 1)).astype(np.int32)
-    return order, cell_start
-
-
 @pytest.mark.parametrize("mode", [0, 1, 2, 3])
 @pytest.mark.parametrize("nox,galerkin,tile,kind", [(3, 1, (8, 8, 8), "sorted"), (3, 1, (8, 8, 8), "moved"),
                                                     (3, 1, (4, 4, 4), "moved"), (1, 1, (8, 8, 8), "moved"),
@@ -354,3 +340,72 @@ def test_bilinear_filter_kernels_under_simt_emulation(orc, npass):
     orc.lib().orc_apply_filter(C.byref(src[0].desc), C.byref(wbig.desc), abi.int3(npass))
     assert hl.pic_apply_filter(C.byref(src[0].desc), C.byref(big.desc), abi.int3(npass), None) == 0, hl.pic_last_error()
     assert rel_linf(big.a, wbig.a) <= 1e-14
+
+
+# ---------------------------------------------------------------------------------------------------------
+# the particle sets of tests/particle_sets.py (steady state, Poisson counts, a full sub-particle queue) through the
+# host library's C ABI: the cell-sorted deposition modes and the supercell gather, against the oracle
+# ---------------------------------------------------------------------------------------------------------
+EMULATED_SETS = ("steady", "poisson", "crowded_movers")
+
+
+@pytest.mark.parametrize("mode", [abi.PIC_DEPOSIT_RUNS, abi.PIC_DEPOSIT_RUNS_SLAB, abi.PIC_DEPOSIT_CELLS,
+                                  abi.PIC_DEPOSIT_CELLS3])
+@pytest.mark.parametrize("nox", [1, 3])
+@pytest.mark.parametrize("name", EMULATED_SETS)
+def test_deposition_modes_on_particle_sets_under_simt_emulation(orc, name, nox, mode):
+    from host_harness import harness
+    hl = harness.host_library()
+    s = ps.get(name)
+    ng = (nox + 2,) * 3
+    xyzmin, lo = s.corner(ng)
+    P = orc.HostParticles(**s.arrays())
+    J = [orc.HostFab(s.box_lo, s.box_hi, ng, abi.YEE_STAG[c]) for c in (6, 7, 8)]
+    K = [orc.HostFab(s.box_lo, s.box_hi, ng, abi.YEE_STAG[c]) for c in (6, 7, 8)]
+    args = (abi.dbl3(s.dinv), abi.dbl3(xyzmin), abi.int3(lo), s.q, s.dt, -0.5 * s.dt, nox)
+    assert orc.lib().orc_deposit_esirkepov(C.byref(P.soa), 0, P.np, orc.fab_array(J), *args) == 0
+    cs = s.cell_start.astype(np.int32)
+    bins = abi.pic_bins()
+    bins.cell_start = cs.ctypes.data
+    for d in range(3):
+        bins.box_lo[d], bins.box_hi[d], bins.tile[d] = s.box_lo[d], s.box_hi[d], ps.TILE
+    bins.np_binned = s.np
+    hl.pic_set_deposit_mode(mode)
+    try:
+        assert hl.pic_deposit_esirkepov(C.byref(P.soa), 0, P.np, orc.fab_array(K), *args, C.byref(bins), None) == 0, \
+            hl.pic_last_error()
+    finally:
+        hl.pic_set_deposit_mode(0)
+    for c in range(3):
+        assert rel_linf(K[c].a, J[c].a) <= 1e-13, "j" + "xyz"[c]
+
+
+@pytest.mark.parametrize("mode", [0, 1])
+@pytest.mark.parametrize("name", EMULATED_SETS + ("scrambled_rows",))
+def test_gather_push_tile_kernels_on_particle_sets_under_simt_emulation(orc, simt, name, mode):
+    s = ps.get(name)
+    nox, galerkin = 3, 1
+    ngEB = (4, 4, 4)
+    xyzmin, lo = s.corner(ngEB)
+    from helpers import random_fields
+    F = random_fields(orc, s.box_lo, s.box_hi, ngEB, 5, comps=range(6), scale=[1e10] * 3 + [30.0] * 3)
+    P = orc.HostParticles(**s.arrays())
+    Q = P.copy()
+    cs = s.cell_start.astype(np.int32)
+    bins = abi.pic_bins()
+    bins.cell_start = cs.ctypes.data
+    for d in range(3):
+        bins.box_lo[d], bins.box_hi[d], bins.tile[d] = s.box_lo[d], s.box_hi[d], ps.TILE
+    bins.np_binned = s.np
+    for push_position in (1, 0):
+        assert simt.simt_gather_push(C.byref(Q.soa), orc.fab_array(F[0:3]), orc.fab_array(F[3:6]), abi.dbl3(s.dinv),
+                                     abi.dbl3(xyzmin), abi.int3(lo), s.q, s.m, s.dt, nox, galerkin,
+                                     abi.PUSHER_BORIS, push_position, C.byref(bins), mode) == 0
+        orc.lib().orc_gather_push(C.byref(P.soa), 0, P.np, orc.fab_array(F[0:3]), orc.fab_array(F[3:6]), abi.dbl3(s.dinv),
+                                  abi.dbl3(xyzmin), abi.int3(lo), s.q, s.m, s.dt, nox, galerkin, abi.PUSHER_BORIS,
+                                  push_position)
+    lx = s.n[0] * s.dx[0]
+    for k in ("x", "y", "z"):
+        assert np.max(np.abs(getattr(Q, k) - getattr(P, k))) <= 1e-13 * lx, k
+    for k in ("ux", "uy", "uz"):
+        assert rel_linf(getattr(Q, k), getattr(P, k)) <= 1e-13, k

@@ -141,10 +141,12 @@ SOLVER_YEE, SOLVER_CKC = 0, 1
 PIC_ERR_ABORT, PIC_ERR_RETURN = 0, 1
 PUSHER_BORIS, PUSHER_VAY, PUSHER_HC = 0, 1, 2
 # pic_set_deposit_mode / pic_set_gather_mode (include/pic_b200.h)
-PIC_DEPOSIT_RUNS, PIC_DEPOSIT_TILE, PIC_DEPOSIT_CELLS, PIC_DEPOSIT_CELLS2, PIC_DEPOSIT_CELLS2_WIDE = 0, 1, 7, 8, 9
+PIC_DEPOSIT_RUNS, PIC_DEPOSIT_TILE, PIC_DEPOSIT_RUNS2, PIC_DEPOSIT_RUNS_SLOTRED = 0, 1, 2, 3
+PIC_DEPOSIT_RUNS2_SLOTRED, PIC_DEPOSIT_RUNS4, PIC_DEPOSIT_RUNS4_SLOTRED = 4, 5, 6
+PIC_DEPOSIT_CELLS, PIC_DEPOSIT_CELLS2, PIC_DEPOSIT_CELLS2_WIDE = 7, 8, 9
 PIC_DEPOSIT_CELLS3, PIC_DEPOSIT_CELLS3_WIDE = 10, 11
 PIC_DEPOSIT_RUNS_SLAB = 12
-PIC_GATHER_TILE, PIC_GATHER_PAIRS, PIC_GATHER_PAIRS_WIDE = 0, 1, 2
+PIC_GATHER_TILE, PIC_GATHER_PAIRS, PIC_GATHER_PAIRS_WIDE, PIC_GATHER_PAIRS_192 = 0, 1, 2, 3
 
 # Yee staggering of WarpX (Source/WarpX.cpp:2117-2125): 1 = nodal.  Order Ex Ey Ez Bx By Bz jx jy jz.
 YEE_STAG = ((0, 1, 1), (1, 0, 1), (1, 1, 0),

@@ -807,6 +807,11 @@ static int launch_cells(SoaView P, long np, const pic_fab J[3], const DepositGeo
     BinsView bins = make_bins(*pb);
     if (bins.tile[0] != T::T || bins.tile[1] != T::T || bins.tile[2] != T::T)
         return fail("pic_deposit_esirkepov(cells): the bins must use 8 x 8 x 8 supercells");
+    // the listed particles go through deposit_general_kernel, whose cell keys take 10 bits per direction: refuse
+    // before the cell kernel has deposited anything (launch_general would refuse only after it)
+    for (int d = 0; d < 3; ++d)
+        for (int c = 0; c < 3; ++c)
+            if (J[c].hi[d] - J[c].lo[d] + 2 > 1022) return fail("pic_deposit_esirkepov: J extent > 1020 points per rank");
     const long np_lim = np < (long)bins.np_limit ? np : (long)bins.np_limit;
     const unsigned grid = (unsigned)(bins.nt[0] * bins.nt[1] * bins.nt[2]);
     J3 j3; j3.v[0] = make_view(J[0]); j3.v[1] = make_view(J[1]); j3.v[2] = make_view(J[2]);
