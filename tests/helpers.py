@@ -22,6 +22,76 @@ def random_fields(orc, box_lo, box_hi, ng, seed, comps=range(6), scale=None):
     return out
 
 
+# ---------------------------------------------------------------------------------------------
+# Gauss's law through the whole step.  Esirkepov deposition gives rho(x^{n+1}) - rho(x^n) = -dt div J to round-off,
+# and EvolveE's downward differences give div E^{n+1} - div E^n = -(dt/ep0) div J (Yee and CKC alike), so
+# G = div E - rho/ep0 is the same at every step on every node of a periodic box.
+# ---------------------------------------------------------------------------------------------
+def gauss_residual(E, rho, dx, n_cell):
+    """G = div E - rho/ep0 on the N^3 unique nodes of a periodic box, as a numpy array or a torch tensor (whichever
+    the inputs are).  E: the valid Ex, Ey, Ez arrays [k, j, i] of the whole box; rho: the valid nodal charge density
+    (guard cells already summed in).  div E at node (i, j, k) is (Ex[i] - Ex[i-1])/dx + (same in y) + (same in z),
+    taken periodically; the upper nodal duplicate is dropped."""
+    xp = np if isinstance(rho, np.ndarray) else __import__("torch")
+    u = tuple(slice(0, n_cell[2 - ax]) for ax in range(3))
+    div = 0.0
+    for d in range(3):
+        e = E[d][u]
+        div = div + (e - xp.roll(e, 1, 2 - d)) / dx[d]
+    return div - rho[u] / workloads.EP0
+
+
+def gauss_drift(G, G0, rho0):
+    """max|G - G0| / max|rho0/ep0|: the change of G over the run, on the scale of the initial charge."""
+    scale = float(abs(rho0).max()) / workloads.EP0
+    return float(abs(G - G0).max()) / scale
+
+
+def div_b_ratio(B, dx, n_cell):
+    """max|div B| / (max|B|/dx) over the N^3 unique cells of a periodic box (B: valid Bx, By, Bz arrays [k, j, i])."""
+    xp = np if isinstance(B[0], np.ndarray) else __import__("torch")
+    u = tuple(slice(0, n_cell[2 - ax]) for ax in range(3))
+    div, scale = 0.0, 0.0
+    for d in range(3):
+        b = B[d][u]
+        div = div + (xp.roll(b, -1, 2 - d) - b) / dx[d]
+        scale = max(scale, float(abs(b).max()) / dx[d])
+    return float(abs(div).max()) / scale if scale > 0 else 0.0
+
+
+def simulation_gauss(sim):
+    """(G, rho) of a one-rank Simulation's current state as tensors on its device: rho from Simulation.rho_numpy
+    (pic_deposit_charge, the filter when it is on, SumBoundary), div E with torch where the fields live."""
+    t = sim.torch
+    E = [sim.data[c][sim.fab[c].valid_slices()] for c in range(3)]
+    d, rho = sim.rho_numpy()
+    rho = t.from_numpy(rho[d.valid_slices()].copy()).to(sim.device)
+    return gauss_residual(E, rho, sim.dx, sim.n_cell), rho
+
+
+def oracle_rho(orc, n_cell, prob_lo, prob_hi, nox, parts, q, use_filter=False, filter_npass=(1, 1, 1)):
+    """Valid nodal charge density [k, j, i] of the particles `parts` (dict x..uz) in the periodic box, computed by the
+    oracle: orc_deposit_charge, then (with the filter) the bilinear filter over the grown box, then SumBoundary --
+    the sequence of Simulation.rho_numpy."""
+    import ctypes as C
+    L = orc.lib()
+    box_lo, box_hi = (0, 0, 0), tuple(v - 1 for v in n_cell)
+    dx = [(prob_hi[d] - prob_lo[d]) / n_cell[d] for d in range(3)]
+    ng = (nox + 2,) * 3
+    rho = orc.HostFab(box_lo, box_hi, ng, (1, 1, 1))
+    xyzmin, lo = lower_corner(prob_lo, dx, box_lo, ng)
+    P = orc.HostParticles(**{k: parts[k] for k in orc.HostParticles.NAMES})
+    assert L.orc_deposit_charge(C.byref(P.soa), C.byref(rho.desc), abi.dbl3([1.0 / v for v in dx]), abi.dbl3(xyzmin),
+                                abi.int3(lo), q, nox) == 0
+    geom = abi.make_geom(n_cell, prob_lo, prob_hi)
+    if use_filter:
+        out = orc.HostFab(box_lo, box_hi, [ng[d] + filter_npass[d] for d in range(3)], (1, 1, 1))
+        L.orc_apply_filter(C.byref(rho.desc), C.byref(out.desc), abi.int3(filter_npass))
+        rho = out
+    L.orc_sum_boundary(C.byref(rho.desc), 1, abi.int3(rho.desc.ng), abi.int3(rho.desc.ng), C.byref(geom))
+    return rho.valid()
+
+
 def make_species_in_box(n_cell, prob_lo, prob_hi, ppc, u_th, seed, perturbation=0.0):
     wl = workloads.uniform_plasma_3d(n_cell=n_cell, ppc=ppc, u_th=u_th, seed=seed,
                                      lx=prob_hi[0] - prob_lo[0], perturbation=perturbation)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """TEST INFRASTRUCTURE -- runs the `-m gpu` test functions (tests/test_gpu_parity.py, tests/test_gpu_particle_sets.py,
-tests/test_gpu_zz_lwfa.py)
+tests/test_gpu_gauss.py, tests/test_gpu_zz_lwfa.py)
 against the HOST build of the library (harness.host_library: every csrc file compiled by g++ against the SIMT emulator),
 for a container without a GPU:
 
@@ -11,6 +11,7 @@ for a container without a GPU:
 The test functions run unchanged, with their own tolerances.  Substitutions: warpx_b200.engine.Simulation -> the host
 subclass of harness.host_simulation_class(); the library loader -> harness.host_library; the `cuda` fixture -> an
 object whose synchronize() does nothing; the `dev` fixture -> the same helper with CPU tensors ("upload" = a copy).
+The Gauss's-law module runs its cases at 16^3 for 8 steps (checkpoints 1, 4, 5, 8) instead of the benchmark's sizes.
 This checks the step sequence, argument builders and kernel arithmetic; it cannot check races, launch bounds or
 speed -- it does not replace the device run, and nothing in the product uses it."""
 import inspect
@@ -65,8 +66,14 @@ class _TorchOnHost:
 
 import test_gpu_parity as TP  # noqa: E402
 import test_gpu_particle_sets as TS  # noqa: E402
+import test_gpu_gauss as TG  # noqa: E402
 import test_gpu_zz_lwfa as TL  # noqa: E402
 from oracle import oracle as orc  # noqa: E402
+
+
+TG.BENCH_N = TG.MODE_N = TG.ORDER_N = 16
+TG.CHECKPOINTS = TG.ORDER_CHECKPOINTS = (1, 4, 5, 8)
+TG.bench_n = lambda t: TG.BENCH_N
 
 
 class HostDev(TP.Dev):
@@ -99,7 +106,7 @@ def main():
     minus = [w[1:] for w in sys.argv[1:] if w.startswith("-")]
     golden = json.load(open(os.path.join(TESTS, "golden", "warpx_checksums.json")))
     npass = nfail = 0
-    for mod in (TP, TS, TL):
+    for mod in (TP, TS, TG, TL):
         for name, fn in sorted(vars(mod).items()):
             if not name.startswith("test_") or not inspect.isfunction(fn) or fn.__module__ != mod.__name__:
                 continue

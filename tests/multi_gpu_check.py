@@ -6,7 +6,8 @@
 
 Config 1 (64^3 Langmuir, 40 steps) on a brick decomposition: WarpX's golden checksums at rtol 1e-9
 (what the reference's own 2-rank CI runs compare, Examples/CMakeLists.txt:98-104), particle-count
-conservation through migration, and an order-3 thermal run compared with the single-box oracle."""
+conservation through migration, an order-3 thermal run compared with the single-box oracle, and Gauss's law over the
+union of the bricks."""
 import ctypes as C
 import json
 import os
@@ -30,7 +31,7 @@ def main():
     torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", rank)))
     dist.init_process_group("nccl", device_id=torch.device("cuda", torch.cuda.current_device()))
     ok = True
-    sections = os.environ.get("PIC_CHECK_SECTIONS", "order3,lwfa,boosted").split(",")     # debugging: skip the slower sections
+    sections = os.environ.get("PIC_CHECK_SECTIONS", "order3,gauss,lwfa,boosted").split(",")     # debugging: skip the slower sections
     golden = json.load(open(os.path.join(ROOT, "tests", "golden", "warpx_checksums.json")))["test_3d_langmuir_multi"]
     L = oracle.lib()
 
@@ -109,6 +110,39 @@ def main():
                   f"B {b:.12e} vs {bo:.12e}; particles {npart}: {'ok' if good else 'FAIL'}")
         sim3.close()
         del sim3
+    # ---------------- Gauss's law over the union of the bricks (tests/test_host_multirank.py: union_gauss) ----------------
+    # (order 3, thermal electrons at u_th = 0.3 c crossing between bricks every step: a particle that migration loses or
+    #  duplicates breaks G = div E - rho/ep0 by about 4e-2 of max|rho^0/ep0|)
+    if "gauss" in sections:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        from helpers import gauss_drift
+        from test_host_multirank import union_gauss, union_state
+        wl = workloads.uniform_plasma_3d(n=n3, ppc=(2, 1, 1), u_th=0.3, lx=5e-6, perturbation=0.01)
+        mine = workloads.uniform_plasma_3d(n=n3, ppc=(2, 1, 1), u_th=0.3, lx=5e-6, perturbation=0.01,
+                                           box_lo=dec3.box_lo, box_hi=dec3.box_hi)
+        s = mine["species"][0]
+        simg = Simulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=3, dist=dist, sort_interval=4)
+        simg.add_species(s["name"], s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
+        done, states = 0, []
+        for step in (0, 1, 4, 5, 12):
+            if step > done:
+                simg.Evolve(step - done, synchronize_last=False)
+                done = step
+            torch.cuda.synchronize()
+            got = [None] * world
+            dist.all_gather_object(got, union_state(simg))
+            states.append(got)
+        if rank == 0:
+            G0, rho0, ids0 = union_gauss(oracle, states[0], wl, 3)
+            for step, st in zip((1, 4, 5, 12), states[1:]):
+                G, _, ids = union_gauss(oracle, st, wl, 3)
+                r = gauss_drift(G, G0, rho0)
+                good = r <= 1e-11 and len(ids[0]) == len(ids0[0]) and np.array_equal(np.sort(ids[0]), np.sort(ids0[0]))
+                ok &= good
+                print(f"[gauss x{world}] step {step}: max|G^n - G^0| / max|rho^0/ep0| {r:.3e}, "
+                      f"{len(ids[0])} particles, ids kept: {'ok' if good else 'FAIL'}")
+        simg.close()
+        del simg
     # ---------------- laser-acceleration deck on z slabs: moving window over several ranks ----------------
     # (PEC walls on the end slabs, neighbour planes pulled in by the window shift, one cell layer of
     #  particles migrating down per shift, injection on the top slab, replicated antenna) against WarpX's

@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 import particle_sets as ps
-from helpers import random_fields, rel_linf
+from helpers import gauss_drift, oracle_rho, random_fields, rel_linf, simulation_gauss
 from test_gpu_parity import Dev, _match_particles, _run_both  # noqa: F401
 from warpx_b200 import abi, workloads
 
@@ -239,7 +239,7 @@ def test_run_kernels_refuse_j_wider_than_their_keys(orc, dev, mode):
 def test_steady_state_loop_matches_oracle(orc, cuda, deposit_mode, gather_mode):
     """`steady` particles (with their log-uniform weights; 16^3 cells: the guard-cell exchange of order 3 needs more
     than 8 cells per axis) handed to the engine and to a fresh oracle, fields zero in both, 12 steps of order 3 with a
-    cell sort every 4: the bar of test_order3_loop_matches_oracle."""
+    cell sort every 4: the bar of test_order3_loop_matches_oracle; and Gauss's law as test_gpu_gauss.py checks it."""
     from warpx_b200.lib import lib as piclib
     s = ps.steady(n=(16, 16, 16))
     wl = dict(n_cell=s.n, prob_lo=s.prob_lo, prob_hi=s.prob_hi,
@@ -264,3 +264,9 @@ def test_steady_state_loop_matches_oracle(orc, cuda, deposit_mode, gather_mode):
         assert np.max(np.abs(A[k] - B[k])) / sim.dx[0] <= 1e-10
     for k in ("ux", "uy", "uz"):
         assert np.max(np.abs(A[k] - B[k])) / workloads.C <= 1e-10
+    # Gauss's law (test_gpu_gauss.py) with these weights: G^0 = -rho^0/ep0 (fields start at zero)
+    G0 = -oracle_rho(orc, s.n, s.prob_lo, s.prob_hi, 3, s.arrays(), s.q) / workloads.EP0
+    G, _ = simulation_gauss(sim)
+    r = gauss_drift(G.cpu().numpy(), G0[:s.n[2], :s.n[1], :s.n[0]], -G0 * workloads.EP0)
+    print("GAUSS steady-state loop, deposit mode %d gather mode %d: %.2e" % (deposit_mode, gather_mode, r))
+    assert r <= 1e-11, r

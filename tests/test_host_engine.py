@@ -188,3 +188,30 @@ def test_checkpoint_restart_on_the_host_continues_the_run(orc, HostSimulation, t
     for k in ("x", "y", "z", "ux", "uy", "uz"):
         scale = ref.dx[0] if k in "xyz" else workloads.C
         assert np.max(np.abs(A[k] - B[k])) / scale <= 1e-11, k
+
+
+@pytest.mark.parametrize("mode", [abi.PIC_DEPOSIT_RUNS, abi.PIC_DEPOSIT_CELLS])
+def test_host_engine_keeps_gauss_law(HostSimulation, mode):
+    """Gauss's law through the C++ driver's whole step (tests/helpers.py: gauss_residual): 16^3 x 8 ppc, order 3, hot
+    enough to cross cell faces every step, 12 steps with a cell sort every 4, in the default deposition and with
+    PIC_DEPOSIT_CELLS.  max|G^n - G^0| / max|rho^0/ep0| <= 1e-12 after steps 1, 4, 5 and 12; the particle count holds."""
+    from helpers import gauss_drift, simulation_gauss
+    from host_harness import harness
+    wl = workloads.uniform_plasma_3d(n=16, ppc=(2, 2, 2), u_th=0.1, lx=2.5e-6)
+    s = wl["species"][0]
+    hl = harness.host_library()
+    hl.pic_set_deposit_mode(mode)
+    try:
+        sim = HostSimulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=3, sort_interval=4)
+        sim.add_species(s["name"], s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
+        assert sim.native
+        G0, rho0 = simulation_gauss(sim)
+        done = 0
+        for step in (1, 4, 5, 12):
+            sim.Evolve(step - done, synchronize_last=False)
+            done = step
+            G, _ = simulation_gauss(sim)
+            assert gauss_drift(G, G0, rho0) <= 1e-12, step
+            assert sim.species[0].np == len(s["x"])
+    finally:
+        hl.pic_set_deposit_mode(abi.PIC_DEPOSIT_RUNS)

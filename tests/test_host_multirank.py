@@ -422,3 +422,89 @@ def test_classify_from_candidate_list_matches_full_sweep(orc, hh):
     assert count[0] == len(store) + 1
     got, gc = run(True, cand)                                                 # overflowed list: every particle is visited
     assert got == want and list(gc) == list(wc)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Gauss's law over the union of the bricks (tests/helpers.py: gauss_residual): a particle that migration loses or
+# duplicates breaks G = div E - rho/ep0 by about 4e-2 of max|rho^0/ep0|.
+# ---------------------------------------------------------------------------------------------------------------------
+def union_state(sim):
+    """What union_gauss needs of one rank: its box, the unique part of its valid E, and its particles."""
+    E = []
+    for c in range(3):
+        d, a = sim.field_numpy(c)
+        nb = [sim.box_hi[ax] - sim.box_lo[ax] + 1 for ax in range(3)]
+        E.append(a[d.valid_slices()][:nb[2], :nb[1], :nb[0]].copy())
+    parts = [{k: v.copy() for k, v in sim.species_numpy(i).items()} for i in range(len(sim.species))]   # host "device" memory
+    return dict(box=(sim.box_lo, sim.box_hi), E=E, parts=parts)
+
+
+def union_gauss(orc, states, full, nox, use_filter=False):
+    """G of the whole box from every rank's state, rho from the oracle's charge deposit of every rank's particles;
+    the first species' rho (the scale of G: a neutral plasma has almost none in total); the union's particle ids."""
+    from helpers import gauss_residual, oracle_rho
+    n = full["n_cell"]
+    E = [np.full((n[2], n[1], n[0]), np.nan) for _ in range(3)]
+    for st in states:
+        lo, hi = st["box"]
+        for c in range(3):
+            E[c][lo[2]:hi[2] + 1, lo[1]:hi[1] + 1, lo[0]:hi[0] + 1] = st["E"][c]
+    assert not any(np.isnan(e).any() for e in E)
+    rho, first, ids = 0.0, None, []
+    for isp, s in enumerate(full["species"]):
+        parts = {k: np.concatenate([st["parts"][isp][k] for st in states]) for k in ("x", "y", "z", "w", "ux", "uy", "uz", "id")}
+        one = oracle_rho(orc, n, full["prob_lo"], full["prob_hi"], nox, parts, s["q"], use_filter)
+        first = one if first is None else first
+        rho = rho + one
+        ids.append(parts["id"])
+    dx = [(full["prob_hi"][d] - full["prob_lo"][d]) / n[d] for d in range(3)]
+    return gauss_residual(E, rho, dx, n), first, ids
+
+
+def gauss_bricks(orc, hh, full, world, nox, checkpoints, **kw):
+    """Run the bricks through the checkpoints and check G of their union at each: max|G^n - G^0| / max|rho^0/ep0|
+    <= 1e-12 (rho^0 of the first species), every particle id exactly once, the particle count kept.  Returns whether particles changed brick."""
+    from helpers import gauss_drift
+    HS = hh.host_simulation_class()
+    n = full["n_cell"]
+
+    def rank_fn(rank, dist):
+        dec = parallel.Decomposition(n, parallel.brick_grid(world), rank)
+        sim = HS(n, full["prob_lo"], full["prob_hi"], nox=nox, dist=dist, sort_interval=4, **kw)
+        for s in full["species"]:
+            cell = [np.floor((s[k] - full["prob_lo"][d]) / sim.dx[d]).astype(int) for d, k in enumerate("xyz")]
+            m = np.ones(len(s["x"]), dtype=bool)
+            for d in range(3):
+                m &= (cell[d] >= dec.box_lo[d]) & (cell[d] <= dec.box_hi[d])
+            sim.add_species(s["name"], s["q"], s["m"], *[s[k][m] for k in ("x", "y", "z", "w", "ux", "uy", "uz")])
+        out, done, mine, moved = [union_state(sim)], 0, sim.species[0].np, False
+        for step in checkpoints:
+            sim.Evolve(step - done, synchronize_last=False)
+            done = step
+            out.append(union_state(sim))
+            moved = moved or sim.species[0].np != mine
+        return dict(states=out, moved=moved)
+
+    res = hh.run_ranks(world, rank_fn)
+    G0, rho0, ids0 = union_gauss(orc, [r["states"][0] for r in res], full, nox, kw.get("use_filter", False))
+    for k, step in enumerate(checkpoints):
+        G, _, ids = union_gauss(orc, [r["states"][k + 1] for r in res], full, nox, kw.get("use_filter", False))
+        for a, b in zip(ids, ids0):
+            assert len(a) == len(b) and np.array_equal(np.sort(a), np.sort(b)), step
+        r = gauss_drift(G, G0, rho0)
+        assert r <= 1e-12, (step, r)
+    return any(r["moved"] for r in res)
+
+
+def test_two_bricks_keep_gauss_law(orc, hh):
+    """Two bricks as in test_two_bricks_periodic_loop_matches_oracle (16^3, order 1), with thermal electrons at
+    u_th = 0.3 c so that particles cross between the bricks every step, 12 steps."""
+    full = workloads.uniform_plasma_3d(n=16, ppc=(2, 1, 1), u_th=0.3, perturbation=0.01)
+    assert gauss_bricks(orc, hh, full, 2, 1, (1, 4, 5, 12))
+
+
+def test_eight_bricks_keep_gauss_law(orc, hh):
+    """The eight-brick loop of test_eight_bricks_order3_thermal_loop_matches_oracle (order 3, bilinear filter, u_th =
+    0.3 c: particles cross to face, edge and corner neighbours), 8 steps."""
+    full = workloads.uniform_plasma_3d(n=16, ppc=(2, 1, 1), u_th=0.3, perturbation=0.01)
+    assert gauss_bricks(orc, hh, full, 8, 3, (1, 4, 5, 8), use_filter=True)

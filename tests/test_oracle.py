@@ -739,3 +739,107 @@ def test_particle_boundaries_golden_checksums(orc, golden):
     sim.evolve(wl["max_step"])
     check_particle_boundaries(golden, sim.particles)
     assert sim.checksum_field(0) == 0.0 and len(sim.particles(1)["x"]) == 1
+
+
+# ---------------------------------------------------------------------------------------------
+# Gauss's law through the whole step (tests/helpers.py: gauss_residual).  G = div E - rho/ep0 must stay what it was at
+# the start on every node.  G cannot see the gather, the push or EvolveB (continuity holds whatever velocity a particle
+# gets, div curl B = 0 for any B); div B = 0 is checked beside it.
+# ---------------------------------------------------------------------------------------------
+GAUSS_ORACLE_TOL = 1e-12
+
+
+def _oracle_gauss(orc, osim, wl, nox, use_filter=False):
+    """(G, rho) of the oracle run's current state; rho from orc_deposit_charge + orc_sum_boundary."""
+    from helpers import gauss_residual, oracle_rho
+    s = wl["species"][0]
+    E = []
+    for c in range(3):
+        d, a = osim.fab(c)
+        E.append(a[d.valid_slices()])
+    rho = oracle_rho(orc, wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox, osim.particles(0), s["q"], use_filter)
+    dx = [(wl["prob_hi"][d] - wl["prob_lo"][d]) / wl["n_cell"][d] for d in range(3)]
+    return gauss_residual(E, rho, dx, wl["n_cell"]), rho
+
+
+@pytest.mark.parametrize("nox,solver,pusher,use_filter,u_th", [
+    (1, abi.SOLVER_YEE, abi.PUSHER_BORIS, False, 0.01), (2, abi.SOLVER_YEE, abi.PUSHER_BORIS, False, 0.01),
+    (3, abi.SOLVER_YEE, abi.PUSHER_BORIS, False, 0.01), (4, abi.SOLVER_YEE, abi.PUSHER_BORIS, False, 0.01),
+    (3, abi.SOLVER_CKC, abi.PUSHER_VAY, False, 0.01), (3, abi.SOLVER_YEE, abi.PUSHER_BORIS, True, 0.01),
+    (1, abi.SOLVER_YEE, abi.PUSHER_BORIS, False, 0.3), (3, abi.SOLVER_CKC, abi.PUSHER_VAY, True, 0.3)])
+def test_oracle_keeps_gauss_law(orc, nox, solver, pusher, use_filter, u_th):
+    """32^3 x 8 ppc, 60 steps: max|G^n - G^0| / max|rho^0/ep0| <= 1e-12 at every checkpoint, and div B = 0 (Yee)."""
+    from helpers import div_b_ratio, gauss_drift
+    wl = workloads.uniform_plasma_3d(n=32, ppc=(2, 2, 2), u_th=u_th, lx=5e-6)
+    s = wl["species"][0]
+    osim = orc.OracleSim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=nox, solver=solver, pusher=pusher,
+                         use_filter=use_filter)
+    osim.add_species(s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
+    G0, rho0 = _oracle_gauss(orc, osim, wl, nox, use_filter)
+    dx = [(wl["prob_hi"][d] - wl["prob_lo"][d]) / wl["n_cell"][d] for d in range(3)]
+    done, moved = 0, 0.0
+    for step in (1, 4, 5, 20, 60):
+        osim.evolve(step - done, synchronize_last=False)
+        done = step
+        G, rho = _oracle_gauss(orc, osim, wl, nox, use_filter)
+        r = gauss_drift(G, G0, rho0)
+        assert r <= GAUSS_ORACLE_TOL, (step, r)
+        if solver == abi.SOLVER_YEE:      # CKC's EvolveB smooths transversely: its B is not free of the Yee divergence
+            B = []
+            for c in range(3, 6):
+                d, a = osim.fab(c)
+                B.append(a[d.valid_slices()])
+            assert div_b_ratio(B, dx, wl["n_cell"]) <= 1e-9, step
+        moved = max(moved, float(np.max(np.abs(rho - rho0)) / np.max(np.abs(rho0))))
+    assert moved > 1e-3           # the charge did move: the check is not comparing a frozen plasma with itself
+
+
+def _periodic_distance(shape, pos_cells):
+    """Distance in cells (max norm, periodic) of every node of a [k, j, i] array from the point pos_cells (x, y, z)."""
+    dist = np.zeros(shape)
+    for ax in range(3):
+        n = shape[2 - ax]
+        d = np.abs(np.arange(n) - pos_cells[ax]) % n
+        d = np.minimum(d, n - d)
+        sh = [1, 1, 1]
+        sh[2 - ax] = n
+        dist = np.maximum(dist, d.reshape(sh))
+    return dist
+
+
+@pytest.mark.parametrize("edit", ["move", "weight"])
+def test_oracle_gauss_check_sees_one_edited_particle(orc, edit):
+    """Negative control: between steps 5 and 6 one particle moves by 0.37 dx (or its weight grows by half) without a
+    current.  Three steps later G differs from G^0 by more than 1e-4 of max|rho^0/ep0| next to that particle, and by
+    no more than the usual round-off everywhere else."""
+    from helpers import gauss_drift
+    nox = 3
+    wl = workloads.uniform_plasma_3d(n=16, ppc=(2, 2, 2), u_th=0.01, lx=2.5e-6)
+    s = wl["species"][0]
+    kw = dict(nox=nox)
+    osim = orc.OracleSim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], **kw)
+    osim.add_species(s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
+    G0, rho0 = _oracle_gauss(orc, osim, wl, nox)
+    osim.evolve(5, synchronize_last=False)
+    assert gauss_drift(_oracle_gauss(orc, osim, wl, nox)[0], G0, rho0) <= GAUSS_ORACLE_TOL
+    # continue in a new oracle run from the same fields and particles, with one particle edited
+    P = osim.particles(0)
+    ip = 1234
+    dx = (wl["prob_hi"][0] - wl["prob_lo"][0]) / wl["n_cell"][0]
+    if edit == "move":
+        P["x"][ip] += 0.37 * dx
+    else:
+        P["w"][ip] *= 1.5
+    nsim = orc.OracleSim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], **kw)
+    nsim.add_species(s["q"], s["m"], *[P[k] for k in ("x", "y", "z", "w", "ux", "uy", "uz")])
+    for c in range(9):
+        nsim.fab(c)[1][...] = osim.fab(c)[1]
+    nsim.evolve(3, synchronize_last=False)
+    G, _ = _oracle_gauss(orc, nsim, wl, nox)
+    scale = float(np.max(np.abs(rho0))) / workloads.EP0
+    err = np.abs(G - G0) / scale
+    Q = nsim.particles(0)
+    at = [(Q[k][ip] - wl["prob_lo"][d]) / dx for d, k in enumerate("xyz")]
+    near = _periodic_distance(G.shape, at) <= nox
+    assert err[near].max() > 1e-4
+    assert err[~near].max() <= GAUSS_ORACLE_TOL
