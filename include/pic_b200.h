@@ -152,6 +152,28 @@ typedef struct pic_plasma_injector {
     double gamma_boost, beta_boost;
 } pic_plasma_injector;
 
+/* Gaussian particle beam of one species (<species>.injection_style = "gaussian_beam",
+ * Source/Initialization/PlasmaInjector.cpp:222-246 + momentum_distribution_type = gaussian / constant / at_rest,
+ * InjectorMomentum.H:60-90).  Every value is a lab-frame value, as in the deck.  rms = x_rms, y_rms, z_rms;
+ * cut = x_cut.. in units of rms (unset: DBL_MAX, the reference's default, PlasmaInjector.H:108-110);
+ * bound_lo/hi = xmin..zmax (+-inf when unset); u_m / u_th = bulk momentum and spread in units of c
+ * (u_th = 0: constant / at_rest); do_focusing with focal_distance = <species>.focal_distance.
+ * Random numbers: a counter-based Philox4x64-10 keyed by seed (not AMReX's stream), see
+ * pic_add_gaussian_beam.  gamma_boost > 1: frame boosted along +z (MapParticletoBoostedFrame, forward
+ * propagation, transverse positions unchanged); gamma_boost <= 1 = lab frame. */
+typedef struct pic_gaussian_beam {
+    double x_m[3], rms[3], cut[3];
+    double bound_lo[3], bound_hi[3];
+    double q_tot;
+    long npart;
+    int do_symmetrize, symmetrization_order;    /* order 4 or 8 */
+    int do_focusing;
+    double focal_distance;
+    double u_m[3], u_th[3];
+    uint64_t seed;
+    double gamma_boost, beta_boost;
+} pic_gaussian_beam;
+
 enum { PIC_ERR_ABORT = 0, PIC_ERR_RETURN = 1 };
 void pic_set_error_mode(int mode);
 const char* pic_last_error(void);
@@ -433,6 +455,34 @@ int pic_laser_antenna_push(const pic_laser_antenna* prm, const double dx[3], con
 long pic_add_plasma(const pic_plasma_injector* inj, const pic_geom* g, const double cell_size[3],
                     const int box_lo[3], const int box_hi[3], const double part_lo[3], const double part_hi[3],
                     const pic_soa* p, long capacity, uint64_t first_id, double t, void* stream);
+
+/* PhysicalParticleContainer::AddGaussianBeam (Source/Particles/PhysicalParticleContainer.cpp:503-677) +
+ * CheckAndAddParticle (:830-853) + MapParticletoBoostedFrame (:456-500) + the Redistribute of InitData (:450-454)
+ * for the beam described by b.  Draw i (0 <= i < npart, npart /= symmetrization_order with do_symmetrize) takes
+ * the Philox4x64-10 blocks 2i and 2i+1 keyed by seed (pic_philox4x64) and turns them into 8 normals
+ * (pic_gaussian_beam_normals); the first six are x, y, z, ux, uy, uz.  A draw inside the bounds and the cuts
+ * gives 1, 4 or 8 particles (the images of do_symmetrize, in the reference's order) of weight
+ * q_tot / (npart charge) / images; in a boosted frame they are mapped to it at t0 = WarpX::gett_new(0).
+ * Redistribute: positions are wrapped along periodic axes of g (oracle semantics, amrex::enforcePeriodic)
+ * and particles outside a non-periodic face (x < prob_lo or x > prob_hi) are dropped.  The particles whose
+ * position then lies in [own_lo, own_hi) (+-inf at the domain's faces) are appended on the device after
+ * p->np, in creation order; the id of a particle is its index in the creation list of a single box
+ * (AddNParticles, WarpXParticleContainer.cpp:163-240), whatever the decomposition.  Deterministic: a count
+ * pass, a scan, a write pass, no atomics.  p = NULL only counts.  Synchronises `stream` (the count is read
+ * back); borrows device scratch of 16 bytes per 64 draws for the duration of the call.  Every precondition
+ * (npart >= 1, rms >= 0, symmetrization order 4 or 8, 0 < beta_boost < 1 when boosted, a non-zero bulk
+ * momentum when focusing, capacity) is checked before anything is written: a failed call leaves p as it was.
+ * Returns the number of particles appended (or that would be), -1 on error. */
+long pic_add_gaussian_beam(const pic_gaussian_beam* b, double charge, const pic_geom* g, const double own_lo[3],
+                           const double own_hi[3], const pic_soa* p, long capacity, double t0, void* stream);
+
+/* The random numbers of pic_add_gaussian_beam, for checking the generator.  pic_philox4x64: out[4 j + c] = word c
+ * of Philox4x64-10 block first_block + j, keyed by (seed, 0), block j taking the counter (j + 1, 0, 0, 0) -- the
+ * stream of numpy.random.Philox(key=seed) after advance(j).  pic_gaussian_beam_normals: out[8 j + c] = normal c
+ * of draw first_draw + j (Box-Muller on the 53-bit uniforms of the draw's two blocks, warpx_b200.workloads).
+ * out: device memory. */
+int pic_philox4x64(uint64_t seed, long first_block, long nblocks, uint64_t* out, void* stream);
+int pic_gaussian_beam_normals(uint64_t seed, long first_draw, long ndraws, double* out, void* stream);
 
 /* w_out[ip] = w[ip] for particles inside [own_lo, own_hi), 0 elsewhere.  Used for containers that are
  * replicated on every rank (laser antennas): each rank deposits only what lies in its own box. */

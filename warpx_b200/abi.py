@@ -68,6 +68,15 @@ class pic_plasma_injector(C.Structure):
                 ("gamma_boost", C.c_double), ("beta_boost", C.c_double)]
 
 
+class pic_gaussian_beam(C.Structure):
+    _fields_ = [("x_m", C.c_double * 3), ("rms", C.c_double * 3), ("cut", C.c_double * 3),
+                ("bound_lo", C.c_double * 3), ("bound_hi", C.c_double * 3), ("q_tot", C.c_double),
+                ("npart", C.c_long), ("do_symmetrize", C.c_int), ("symmetrization_order", C.c_int),
+                ("do_focusing", C.c_int), ("focal_distance", C.c_double),
+                ("u_m", C.c_double * 3), ("u_th", C.c_double * 3), ("seed", C.c_uint64),
+                ("gamma_boost", C.c_double), ("beta_boost", C.c_double)]
+
+
 FIELD_PERIODIC, FIELD_PEC = 0, 1
 PARTICLE_PERIODIC, PARTICLE_ABSORBING, PARTICLE_REFLECTING = 0, 1, 2
 _FIELD_BC = {"periodic": FIELD_PERIODIC, "pec": FIELD_PEC}
@@ -115,6 +124,31 @@ def make_injector(ppc, bound_lo, bound_hi, density, do_continuous_injection=Fals
     return inj
 
 
+DBL_MAX = 1.7976931348623157e308
+
+
+def make_gaussian_beam(x_m, rms, npart, q_tot, u_m=(0.0, 0.0, 0.0), u_th=(0.0, 0.0, 0.0), cut=(DBL_MAX,) * 3,
+                       bound_lo=(-np.inf,) * 3, bound_hi=(np.inf,) * 3, do_symmetrize=False, symmetrization_order=4,
+                       focal_distance=None, seed=0, gamma_boost=1.0, do_backward_propagation=False):
+    """<species>.injection_style = "gaussian_beam" by the deck's names: x_m = (x_m, y_m, z_m), rms = (x_rms, y_rms,
+    z_rms), cut = (x_cut, y_cut, z_cut) in units of rms, bound_lo/hi = xmin..zmax, u_m / u_th in units of c,
+    focal_distance set = do_focusing.  do_backward_propagation is refused: no deck of the project uses it."""
+    if do_backward_propagation:
+        raise NotImplementedError("gaussian_beam: do_backward_propagation is not supported")
+    b = pic_gaussian_beam()
+    for d in range(3):
+        b.x_m[d], b.rms[d], b.cut[d] = float(x_m[d]), float(rms[d]), float(cut[d])
+        b.bound_lo[d], b.bound_hi[d] = float(bound_lo[d]), float(bound_hi[d])
+        b.u_m[d], b.u_th[d] = float(u_m[d]), float(u_th[d])
+    b.npart, b.q_tot = int(npart), float(q_tot)
+    b.do_symmetrize, b.symmetrization_order = (1 if do_symmetrize else 0), int(symmetrization_order)
+    b.do_focusing = 0 if focal_distance is None else 1
+    b.focal_distance = 0.0 if focal_distance is None else float(focal_distance)
+    b.seed = int(seed)
+    b.gamma_boost, b.beta_boost = float(gamma_boost), beta_of_gamma(gamma_boost)
+    return b
+
+
 def LWFA_SIGNATURES(fabp, soap, gp, bp, lp, jp, dp, ip, vp):
     """ctypes signatures of the non-periodic-domain entry points of include/pic_b200.h."""
     return {
@@ -125,6 +159,10 @@ def LWFA_SIGNATURES(fabp, soap, gp, bp, lp, jp, dp, ip, vp):
         "pic_laser_antenna_particles": (C.c_long, [lp, dp, dp, dp, vp, vp, vp, vp, C.c_long]),
         "pic_laser_antenna_push": (C.c_int, [lp, dp, soap, C.c_double, C.c_double, vp]),
         "pic_add_plasma": (C.c_long, [jp, gp, dp, ip, ip, dp, dp, soap, C.c_long, C.c_uint64, C.c_double, vp]),
+        "pic_add_gaussian_beam": (C.c_long, [C.POINTER(pic_gaussian_beam), C.c_double, gp, dp, dp, soap, C.c_long,
+                                             C.c_double, vp]),
+        "pic_philox4x64": (C.c_int, [C.c_uint64, C.c_long, C.c_long, vp, vp]),
+        "pic_gaussian_beam_normals": (C.c_int, [C.c_uint64, C.c_long, C.c_long, vp, vp]),
         "pic_particles_owned_weights": (C.c_int, [soap, dp, dp, vp, vp]),
         "pic_deposit_charge": (C.c_int, [soap, C.c_long, C.c_long, fabp, dp, dp, ip, C.c_double, C.c_int, vp]),
         "pic_apply_pec_rho": (C.c_int, [fabp, gp, bp, vp]),

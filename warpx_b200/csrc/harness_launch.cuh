@@ -20,6 +20,9 @@ namespace pic {
 static inline void dev_copy(void* dst, const void* src, size_t bytes, void*) { memcpy(dst, src, bytes); }
 static inline void dev_zero(void* dst, size_t bytes, void*) { memset(dst, 0, bytes); }
 static inline bool launched_ok(const char*) { return true; }
+static inline void* dev_alloc(size_t bytes) { return malloc(bytes ? bytes : 1); }
+static inline void dev_free(void* p) { free(p); }
+static inline bool copy_sync(void* dst, const void* src, size_t bytes, void*) { memcpy(dst, src, bytes); return true; }
 #else
 #define PIC_LAUNCH(kernel, body, args, total, stream) \
     do { if ((total) > 0) { kernel<<<(unsigned)(((total) + 255) / 256), 256, 0, (cudaStream_t)(stream)>>>(args); count_launch(); } } while (0)
@@ -28,6 +31,17 @@ static inline void dev_copy(void* dst, const void* src, size_t bytes, void* s) {
 }
 static inline void dev_zero(void* dst, size_t bytes, void* s) { cudaMemsetAsync(dst, 0, bytes, (cudaStream_t)s); }
 static inline bool launched_ok(const char* what) { return check_launch(what); }
+// Scratch for the duration of one call (initial conditions only, never on the step path)
+static inline void* dev_alloc(size_t bytes) {
+    void* p = nullptr;
+    return cudaMalloc(&p, bytes ? bytes : 1) == cudaSuccess ? p : nullptr;
+}
+static inline void dev_free(void* p) { cudaFree(p); }
+// Host <-> device copy on the stream, then wait for it (the caller needs the data now)
+static inline bool copy_sync(void* dst, const void* src, size_t bytes, void* s) {
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, (cudaStream_t)s) == cudaSuccess &&
+           cudaStreamSynchronize((cudaStream_t)s) == cudaSuccess;
+}
 #endif
 
 PIC_HD int slot_add(int* c) {

@@ -484,3 +484,120 @@ extern "C" int pic_particles_boundary_compact(const pic_soa* p, int* work, int c
     PIC_LAUNCH(compact_move_kernel, compact_move_body, a, (long)n_lost, stream);
     return launched_ok("pic_particles_boundary_compact") ? 0 : 1;
 }
+
+// ---------------------------------------------------------------------------------------------
+// Gaussian beam (AddGaussianBeam + CheckAndAddParticle + MapParticletoBoostedFrame + InitData's Redistribute);
+// the per-draw arithmetic is in lwfa_body.cuh.  Not on the step path: runs once, at start-up.
+namespace pic {
+__global__ void beam_count_kernel(BeamArgs a) {
+    const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < a.nchunk) beam_count_body(t, a);
+}
+__global__ void beam_write_kernel(BeamArgs a) {
+    const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < a.nchunk) beam_write_body(t, a);
+}
+
+struct PhiloxArgs { uint64_t seed; long first, n; uint64_t* raw; double* normals; };
+PIC_HD void philox_body(long j, const PhiloxArgs& a) {
+    uint64_t w[4];
+    philox4x64_10(a.seed, (uint64_t)(a.first + j), w);
+    for (int c = 0; c < 4; ++c) a.raw[4 * j + c] = w[c];
+}
+PIC_HD void normals_body(long j, const PhiloxArgs& a) { beam_normals(a.seed, a.first + j, a.normals + 8 * j); }
+__global__ void philox_kernel(PhiloxArgs a) {
+    const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < a.n) philox_body(t, a);
+}
+__global__ void normals_kernel(PhiloxArgs a) {
+    const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < a.n) normals_body(t, a);
+}
+}  // namespace pic
+
+extern "C" int pic_philox4x64(uint64_t seed, long first_block, long nblocks, uint64_t* out, void* stream) {
+    PIC_REQUIRE(first_block >= 0 && nblocks >= 0, "pic_philox4x64: negative block range");
+    PhiloxArgs a{seed, first_block, nblocks, out, nullptr};
+    PIC_LAUNCH(philox_kernel, philox_body, a, a.n, stream);
+    return launched_ok("pic_philox4x64") ? 0 : 1;
+}
+
+extern "C" int pic_gaussian_beam_normals(uint64_t seed, long first_draw, long ndraws, double* out, void* stream) {
+    PIC_REQUIRE(first_draw >= 0 && ndraws >= 0, "pic_gaussian_beam_normals: negative draw range");
+    PhiloxArgs a{seed, first_draw, ndraws, nullptr, out};
+    PIC_LAUNCH(normals_kernel, normals_body, a, a.n, stream);
+    return launched_ok("pic_gaussian_beam_normals") ? 0 : 1;
+}
+
+extern "C" long pic_add_gaussian_beam(const pic_gaussian_beam* b, double charge, const pic_geom* g, const double own_lo[3],
+                                      const double own_hi[3], const pic_soa* p, long capacity, double t0, void* stream) {
+    // preconditions first: a refused call writes nothing
+    if (b->npart < 1) { fail("pic_add_gaussian_beam: npart must be >= 1"); return -1; }
+    for (int d = 0; d < 3; ++d)
+        if (!(b->rms[d] >= 0.0)) { fail("pic_add_gaussian_beam: rms[%d] must be >= 0", d); return -1; }
+    if (b->do_symmetrize && b->symmetrization_order != 4 && b->symmetrization_order != 8) {   // PlasmaInjector.cpp:240-243
+        fail("pic_add_gaussian_beam: symmetrization_order must be 4 or 8"); return -1;
+    }
+    const bool boosted = b->gamma_boost > 1.;
+    if (boosted && !(b->beta_boost > 0. && b->beta_boost < 1.)) { fail("pic_add_gaussian_beam: gamma_boost > 1 needs 0 < beta_boost < 1"); return -1; }
+    BeamArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.images = b->do_symmetrize ? b->symmetrization_order : 1;
+    a.ndraw = b->do_symmetrize ? b->npart / b->symmetrization_order : b->npart;      // npart /= symmetrization_order (:530-532)
+    if (a.ndraw < 1) { fail("pic_add_gaussian_beam: npart %ld < symmetrization_order", b->npart); return -1; }
+    a.seed = b->seed;
+    for (int d = 0; d < 3; ++d) {
+        a.x_m[d] = b->x_m[d]; a.rms[d] = b->rms[d]; a.cut[d] = b->cut[d];
+        a.blo[d] = b->bound_lo[d]; a.bhi[d] = b->bound_hi[d];
+        a.u_m[d] = b->u_m[d]; a.u_th[d] = b->u_th[d];
+        a.periodic[d] = g->periodic[d];
+        a.plo[d] = g->prob_lo[d]; a.phi[d] = g->prob_hi[d]; a.len[d] = g->prob_hi[d] - g->prob_lo[d];
+        a.own_lo[d] = own_lo[d]; a.own_hi[d] = own_hi[d];
+    }
+    a.do_focusing = b->do_focusing ? 1 : 0;
+    if (a.do_focusing) {                                  // focal plane from the bulk momentum (:560-572)
+        const double un = std::sqrt(b->u_m[0] * b->u_m[0] + b->u_m[1] * b->u_m[1] + b->u_m[2] * b->u_m[2]);
+        if (!(un > 0.0)) { fail("pic_add_gaussian_beam: focusing needs a non-zero bulk momentum u_m"); return -1; }
+        for (int d = 0; d < 3; ++d) a.nf[d] = b->u_m[d] / un;
+        for (int d = 0; d < 3; ++d) a.xf[d] = b->x_m[d] + b->focal_distance * a.nf[d];
+    }
+    const double weight = b->q_tot / (a.ndraw * charge);                             // :538
+    a.weight = a.images == 8 ? weight / 8.0 : (a.images == 4 ? weight / 4.0 : weight);
+    a.boosted = boosted ? 1 : 0;
+    a.gamma_boost = boosted ? b->gamma_boost : 1.0;
+    a.uz_boost = boosted ? b->gamma_boost * b->beta_boost * C_LIGHT : 0.0;         // :465
+    a.t0 = t0;
+    a.chunk = 64;
+    a.nchunk = (a.ndraw + a.chunk - 1) / a.chunk;
+    // count pass -> exclusive scan of the per-chunk counts (host, in chunk order) -> write pass
+    const size_t bytes = sizeof(long) * 2 * (size_t)a.nchunk;
+    long* counts = static_cast<long*>(dev_alloc(bytes));
+    if (!counts) { fail("pic_add_gaussian_beam: cannot allocate %zu B of scratch", bytes); return -1; }
+    std::vector<long> h(2 * (size_t)a.nchunk);
+    a.counts = counts;
+    PIC_LAUNCH(beam_count_kernel, beam_count_body, a, a.nchunk, stream);
+    if (!launched_ok("pic_add_gaussian_beam") || !copy_sync(h.data(), counts, bytes, stream)) {
+        dev_free(counts); fail("pic_add_gaussian_beam: count pass failed"); return -1;
+    }
+    long acc = 0, own = 0;
+    for (long c = 0; c < a.nchunk; ++c) {
+        const long ca = h[2 * c], co = h[2 * c + 1];
+        h[2 * c] = acc; h[2 * c + 1] = own;
+        acc += ca; own += co;
+    }
+    if (p == nullptr) { dev_free(counts); return own; }
+    if (p->np + own > capacity) {
+        dev_free(counts);
+        fail("pic_add_gaussian_beam: %ld + %ld particles exceed the capacity %ld", (long)p->np, own, capacity);
+        return -1;
+    }
+    if (own > 0) {
+        a.P = make_soa(*p, p->np);
+        a.id = p->idcpu ? p->idcpu + p->np : nullptr;
+        if (!copy_sync(counts, h.data(), bytes, stream)) { dev_free(counts); fail("pic_add_gaussian_beam: upload failed"); return -1; }
+        PIC_LAUNCH(beam_write_kernel, beam_write_body, a, a.nchunk, stream);
+        if (!launched_ok("pic_add_gaussian_beam")) { dev_free(counts); return -1; }
+    }
+    dev_free(counts);                                     // cudaFree waits for the write pass
+    return own;
+}

@@ -273,5 +273,170 @@ PIC_HD bool boundary_body(long ip, const BoundaryArgs& a) {          // returns 
     return lost;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Gaussian beam (AddGaussianBeam, PhysicalParticleContainer.cpp:503-677).  The reference draws from AMReX's
+// per-thread stream; here draw i takes the counter-based Philox4x64-10 blocks 2i and 2i+1, so that every
+// decomposition (and the numpy reference, warpx_b200.workloads.beam_normals) sees the same draws.
+// Philox4x64-10 of Random123 (Salmon et al., SC'11): 10 rounds, multipliers M0/M1, Weyl key increments W0/W1.
+// Block j = the output of numpy.random.Philox(key=seed) after advance(j): counter (j + 1, 0, 0, 0), key (seed, 0).
+PIC_HD uint64_t mulhi64(uint64_t a, uint64_t b) {
+#ifdef __CUDA_ARCH__
+    return __umul64hi(a, b);
+#else
+    return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+
+PIC_HD void philox4x64_10(uint64_t seed, uint64_t block, uint64_t out[4]) {
+    const uint64_t M0 = 0xD2E7470EE14C6C93ull, M1 = 0xCA5A826395121157ull;
+    const uint64_t W0 = 0x9E3779B97F4A7C15ull, W1 = 0xBB67AE8584CAA73Bull;
+    uint64_t c0 = block + 1, c1 = 0, c2 = 0, c3 = 0, k0 = seed, k1 = 0;
+    for (int r = 0; r < 10; ++r) {
+        if (r > 0) { k0 += W0; k1 += W1; }
+        const uint64_t hi0 = mulhi64(M0, c0), lo0 = M0 * c0;
+        const uint64_t hi1 = mulhi64(M1, c2), lo1 = M1 * c2;
+        const uint64_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
+        c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
+    }
+    out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
+}
+
+// Four normals of one block, as workloads.philox_normal forms them: 53-bit uniforms u in [0, 1), radii from
+// u1 = 1 - u of words 0 and 1, angles 2 pi u of words 2 and 3: (r0 cos, r0 sin, r1 cos, r1 sin).
+PIC_HD void box_muller4(const uint64_t w[4], double* g) {
+    constexpr double TWO_PI = 2.0 * 3.14159265358979323846;
+    double r[2], s[2], c[2];
+    for (int k = 0; k < 2; ++k) {
+        const double u1 = 1.0 - (double)(w[k] >> 11) * (1.0 / 9007199254740992.0);
+        r[k] = sqrt(-2.0 * log(u1));
+        const double th = TWO_PI * ((double)(w[2 + k] >> 11) * (1.0 / 9007199254740992.0));
+#ifdef __CUDA_ARCH__
+        sincos(th, &s[k], &c[k]);
+#else
+        s[k] = sin(th); c[k] = cos(th);
+#endif
+    }
+    g[0] = r[0] * c[0]; g[1] = r[0] * s[0]; g[2] = r[1] * c[1]; g[3] = r[1] * s[1];
+}
+
+PIC_HD void beam_normals(uint64_t seed, long draw, double g[8]) {
+    uint64_t w[4];
+    philox4x64_10(seed, 2 * (uint64_t)draw, w);
+    box_muller4(w, g);
+    philox4x64_10(seed, 2 * (uint64_t)draw + 1, w);
+    box_muller4(w, g + 4);
+}
+
+// Host-built argument block.  The draws are cut into chunks of `chunk`; thread c walks chunk c in order, so
+// that a count pass, an exclusive scan of the per-chunk counts and a write pass give every particle its slot
+// and its id without atomics.
+struct BeamArgs {
+    SoaView P;                       // write pass: already offset to the first free slot
+    uint64_t* id;                    // idem (may be null)
+    long* counts;                    // 2 per chunk: accepted draws, owned particles (count pass: out; write pass:
+                                     // the exclusive prefix sums, in)
+    long ndraw, chunk, nchunk;
+    uint64_t seed;
+    int images;                      // 1, 4 or 8 particles per accepted draw
+    double x_m[3], rms[3], cut[3], blo[3], bhi[3];
+    double u_m[3], u_th[3];
+    int do_focusing;
+    double nf[3], xf[3];             // focusing: unit bulk direction, focal point (:561-572)
+    double weight;                   // per image
+    int boosted;
+    double gamma_boost, uz_boost, t0;
+    int periodic[3];
+    double plo[3], phi[3], len[3];   // problem domain at start-up
+    double own_lo[3], own_hi[3];
+};
+
+// Draw i: position, cuts, momentum, focusing, u *= c (:535-597).  False when the draw is rejected.
+PIC_HD bool beam_base(long i, const BeamArgs& a, double b[6]) {
+    double g[8];
+    beam_normals(a.seed, i, g);
+    double x[3], u[3];
+    for (int d = 0; d < 3; ++d) x[d] = add_rn(a.x_m[d], mul_rn(a.rms[d], g[d]));     // RandomNormal(x_m, x_rms)
+    for (int d = 0; d < 3; ++d)                                                      // insideBounds + cuts (:546-549)
+        if (!(x[d] < a.bhi[d] && x[d] >= a.blo[d] && fabs(sub_rn(x[d], a.x_m[d])) <= mul_rn(a.cut[d], a.rms[d])))
+            return false;
+    for (int d = 0; d < 3; ++d) u[d] = add_rn(a.u_m[d], mul_rn(a.u_th[d], g[3 + d]));   // InjectorMomentumGaussian
+    if (a.do_focusing) {                                                              // :559-593
+        const double gamma = sqrt(add_rn(1.0, add_rn(add_rn(mul_rn(u[0], u[0]), mul_rn(u[1], u[1])), mul_rn(u[2], u[2]))));
+        double v[3];
+        for (int d = 0; d < 3; ++d) v[d] = mul_rn(u[d] / gamma, C_LIGHT);
+        const double v_dot_n = add_rn(add_rn(mul_rn(v[0], a.nf[0]), mul_rn(v[1], a.nf[1])), mul_rn(v[2], a.nf[2]));
+        const double t = add_rn(add_rn(mul_rn(sub_rn(a.xf[0], x[0]), a.nf[0]), mul_rn(sub_rn(a.xf[1], x[1]), a.nf[1])),
+                                mul_rn(sub_rn(a.xf[2], x[2]), a.nf[2])) / v_dot_n;
+        for (int d = 0; d < 3; ++d) x[d] = sub_rn(x[d], mul_rn(sub_rn(v[d], mul_rn(v_dot_n, a.nf[d])), t));
+    }
+    for (int d = 0; d < 3; ++d) { b[d] = x[d]; b[3 + d] = mul_rn(u[d], C_LIGHT); }
+    return true;
+}
+
+// Image k of an accepted draw (:598-631: (x,y) (x,-y) (-x,y) (-x,-y), then (y,x) (-y,x) (y,-x) (-y,-x), u alike),
+// CheckAndAddParticle (:830-853) -> MapParticletoBoostedFrame (:456-500, t_lab = 0), then the Redistribute of
+// InitData: the periodic wrap and the drop beyond a non-periodic face.  True when the particle is this rank's.
+PIC_HD bool beam_image(int k, const double b[6], const BeamArgs& a, double q[6]) {
+    const bool swap = k >= 4, fa = swap ? (k & 1) : (k & 2), fb = swap ? (k & 2) : (k & 1);
+    const double A = swap ? b[1] : b[0], B = swap ? b[0] : b[1];
+    const double uA = swap ? b[4] : b[3], uB = swap ? b[3] : b[4];
+    q[0] = fa ? -A : A; q[1] = fb ? -B : B; q[2] = b[2];
+    q[3] = fa ? -uA : uA; q[4] = fb ? -uB : uB; q[5] = b[5];
+    if (a.boosted) {
+        constexpr double C2 = C_LIGHT * C_LIGHT;
+        const double z = q[2], ux = q[3], uy = q[4], uz = q[5];
+        const double tpr = sub_rn(0.0, mul_rn(a.uz_boost, z) / C2);                   // gamma_boost t_lab = 0
+        const double zpr = mul_rn(a.gamma_boost, z);
+        const double uxy2 = add_rn(mul_rn(ux, ux), mul_rn(uy, uy));
+        const double gamma_lab = sqrt(add_rn(1.0, add_rn(uxy2, mul_rn(uz, uz)) / C2));
+        const double uzp = sub_rn(mul_rn(a.gamma_boost, uz), mul_rn(a.uz_boost, gamma_lab));
+        const double gammapr = sqrt(add_rn(1.0, add_rn(uxy2, mul_rn(uzp, uzp)) / C2));
+        q[2] = sub_rn(zpr, mul_rn(sub_rn(tpr, a.t0), uzp / gammapr));
+        q[5] = uzp;
+    }
+    bool mine = true;
+    for (int d = 0; d < 3; ++d) {
+        double v = q[d];
+        if (a.periodic[d]) {                                                           // amrex::enforcePeriodic
+            if (v > a.phi[d]) { while (v > a.phi[d]) v = sub_rn(v, a.len[d]); if (v < a.plo[d]) v = a.plo[d]; }
+            else if (v < a.plo[d]) { while (v < a.plo[d]) v = add_rn(v, a.len[d]); if (v > a.phi[d]) v = a.phi[d]; }
+            q[d] = v;
+        } else if (v < a.plo[d] || v > a.phi[d]) {
+            return false;                                                              // outside the domain: no owner
+        }
+        mine = mine && v >= a.own_lo[d] && v < a.own_hi[d];
+    }
+    return mine;
+}
+
+PIC_HD void beam_count_body(long c, const BeamArgs& a) {
+    const long i1 = (c + 1) * a.chunk < a.ndraw ? (c + 1) * a.chunk : a.ndraw;
+    long acc = 0, own = 0;
+    double b[6], q[6];
+    for (long i = c * a.chunk; i < i1; ++i) {
+        if (!beam_base(i, a, b)) continue;
+        ++acc;
+        for (int k = 0; k < a.images; ++k) own += beam_image(k, b, a, q) ? 1 : 0;
+    }
+    a.counts[2 * c] = acc; a.counts[2 * c + 1] = own;
+}
+
+PIC_HD void beam_write_body(long c, const BeamArgs& a) {
+    const long i1 = (c + 1) * a.chunk < a.ndraw ? (c + 1) * a.chunk : a.ndraw;
+    long acc = a.counts[2 * c], slot = a.counts[2 * c + 1];
+    double b[6], q[6];
+    for (long i = c * a.chunk; i < i1; ++i) {
+        if (!beam_base(i, a, b)) continue;
+        for (int k = 0; k < a.images; ++k) {
+            if (!beam_image(k, b, a, q)) continue;
+            a.P.x[slot] = q[0]; a.P.y[slot] = q[1]; a.P.z[slot] = q[2]; a.P.w[slot] = a.weight;
+            a.P.ux[slot] = q[3]; a.P.uy[slot] = q[4]; a.P.uz[slot] = q[5];
+            if (a.id) a.id[slot] = (uint64_t)(acc * a.images + k);
+            ++slot;
+        }
+        ++acc;
+    }
+}
+
 }  // namespace pic
 #endif

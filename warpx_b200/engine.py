@@ -467,6 +467,36 @@ class Simulation:
         self._sync_from_native()
         return sp
 
+    def add_beam_species(self, name, q, m, beam, capacity):
+        """A Gaussian beam (abi.pic_gaussian_beam, <species>.injection_style = "gaussian_beam") created on the device by
+        pic_add_gaussian_beam (PhysicalParticleContainer::AddGaussianBeam + InitData, PhysicalParticleContainer.cpp:
+        450-454,503-677), in the lab frame or mapped into this run's boosted frame at the current time.  Each rank keeps
+        the particles of its own brick; ids are creation indices, the same on any decomposition.  A beam is created
+        once and never refilled.  capacity: entries of every particle array (the run must never exceed it)."""
+        if not self.native:
+            raise NotImplementedError("beam species need the C++ driver")
+        beam.gamma_boost, beam.beta_boost = self.gamma_boost, self.beta_boost
+        empty = np.empty(0)
+        sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity))
+        soa = sp.soa(0)
+        # this brick's half-open share of the domain; the domain's own faces are open (the library drops or wraps there)
+        own_lo = [self.prob_lo[d] + self.dx[d] * self.box_lo[d] if self.box_lo[d] > 0 else -math.inf for d in range(3)]
+        own_hi = [self.prob_lo[d] + self.dx[d] * (self.box_hi[d] + 1) if self.box_hi[d] < self.n_cell[d] - 1 else math.inf
+                  for d in range(3)]
+        n = self.L.pic_add_gaussian_beam(C.byref(beam), q, C.byref(self.geom), abi.dbl3(own_lo), abi.dbl3(own_hi),
+                                         C.byref(soa), sp.capacity, self.time, self.stream)
+        if n < 0:
+            raise RuntimeError("pic_b200: " + self.L.pic_last_error().decode())
+        sp.np = int(n)
+        self.species.append(sp)
+        self._alloc_sort_scratch(sp)
+        a, b = sp.soa(0), sp.soa(1)
+        check(self.L.pic_engine_add_species(self.native, q, m, C.byref(a), C.byref(b), sp.capacity,
+                                            sp.cell_start.data_ptr(), abi.int3(self.tile), sp.work.data_ptr(),
+                                            self.stream))
+        self._sync_from_native()
+        return sp
+
     def add_laser(self, laser):
         """lasers.names / <laser>.*: a Gaussian antenna (LaserParticleContainer ctor + InitData,
         LaserParticleContainer.cpp:84-270,369-560).  The antenna particles are generated on the host like

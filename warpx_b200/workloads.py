@@ -9,6 +9,10 @@ BASELINE.json so that the oracle and the CUDA engine start from bit-identical ar
 * weights: ``w = n * dx*dy*dz / ppc`` (Source/Particles/AddPlasmaUtilities.H:73-77,
   PhysicalParticleContainer.cpp:1275-1288);
 * momenta: ``u = (gamma*beta) * c`` (PhysicalParticleContainer.cpp:1271-1273).
+
+Where the reference draws random numbers from AMReX's stream (config 2's thermal momenta, config 4's Gaussian beam),
+a counter-based Philox4x64-10 generator keyed by a seed replaces it (philox_normal, beam_normals), so that every
+decomposition, the oracle and the device see the same draws.  AMReX's own stream is not reproduced.
 """
 import numpy as np
 
@@ -87,6 +91,26 @@ def philox_normal(seed, first_id, count, ncomp=3):
         for c in range(ncomp):
             out[b:b + n, c] = g[c]
     return out
+
+
+def philox_blocks(seed, first_block, nblocks):
+    """Raw Philox4x64-10 words, shape (nblocks, 4): block j = numpy Philox(key=seed) after advance(j)."""
+    bg = np.random.Philox(key=seed)
+    bg.advance(int(first_block))
+    return bg.random_raw(4 * int(nblocks)).reshape(int(nblocks), 4)
+
+
+def beam_normals(seed, first_draw, count):
+    """The 8 N(0,1) numbers of each Gaussian-beam draw (pic_add_gaussian_beam), shape (count, 8): draw i takes
+    blocks 2i and 2i+1 and turns each into two Box-Muller pairs exactly as philox_normal does (53-bit uniforms,
+    u1 = 1 - u): (r0 cos th0, r0 sin th0, r1 cos th1, r1 sin th1).  Columns 0-5 are x, y, z, ux, uy, uz."""
+    raw = philox_blocks(seed, 2 * int(first_draw), 2 * int(count)).reshape(int(count), 2, 4)
+    u = (raw >> np.uint64(11)).astype(np.float64) * (1.0 / 9007199254740992.0)
+    r = np.sqrt(-2.0 * np.log(1.0 - u[:, :, 0:2]))
+    th = 2.0 * np.pi * u[:, :, 2:4]
+    g = np.stack((r[:, :, 0] * np.cos(th[:, :, 0]), r[:, :, 0] * np.sin(th[:, :, 0]),
+                  r[:, :, 1] * np.cos(th[:, :, 1]), r[:, :, 1] * np.sin(th[:, :, 1])), axis=2)
+    return np.ascontiguousarray(g.reshape(int(count), 8))
 
 
 def uniform_plasma_3d(n=256, ppc=(2, 2, 2), lx=40.0e-6, density=1.0e25, u_th=0.01,
@@ -181,17 +205,23 @@ def max_step_boost_accelerator(zmax_plasma, zmin_domain_boost, gamma_boost, movi
 
 
 def laser_acceleration_boosted_3d(n_cell=(16, 16, 128), max_step=60, gamma_boost=10.0, density=1.e23,
-                                  use_fdtd_nci_corr=False):
+                                  use_fdtd_nci_corr=False, beam=False):
     """BASELINE.json config 4 in the small: Examples/Tests/boosted_diags/
     inputs_test_3d_laser_acceleration_btd (CKC, Vay, order 3, bilinear filter, z moving window at c, PEC in
     z, Gaussian antenna, electrons + ions at rest in the lab with continuous injection, gamma_boost = 10)
-    without the Gaussian beam (AMReX RNG) and the back-transformed diagnostics, on a grid fine enough for
-    omega_p dt < 1 (the regression deck itself runs at omega_p dt = 4.4).  prob_lo / prob_hi below are the
-    boosted-frame values; everything under species / lasers is lab-frame, as in the deck."""
+    without the back-transformed diagnostics, on a grid fine enough for omega_p dt < 1 (the regression deck
+    itself runs at omega_p dt = 4.4).  prob_lo / prob_hi below are the boosted-frame values; everything under
+    species / lasers / beams is lab-frame, as in the deck.  beam=True adds the deck's witness beam under
+    "beams" (keyword arguments of abi.make_gaussian_beam plus name, q, m): its draws come from the
+    counter-based generator of beam_normals, not AMReX's, so the deck's own checksums stay out of reach."""
     M_P = 1.67262192369e-27
     lo, hi = boosted_domain((-128.e-6, -128.e-6, -40.e-6), (128.e-6, 128.e-6, 0.0), gamma_boost, 1.0)
     bounds = dict(bound_lo=(-120.e-6, -120.e-6, 0.0), bound_hi=(120.e-6, 120.e-6, .003))
-    return dict(
+    extra = {}
+    if beam:
+        extra["beams"] = [dict(name="beam", q=-Q_E, m=M_E, x_m=(0.0, 0.0, -20.e-6), rms=(1.e-6, 1.e-6, .2e-6),
+                               npart=1000, q_tot=-1.e-14, u_m=(0.0, 0.0, 200000.), u_th=(.2, .2, 20.))]
+    return dict(**extra,
         n_cell=tuple(n_cell), prob_lo=lo, prob_hi=hi, gamma_boost=gamma_boost,
         field_lo=("periodic", "periodic", "pec"), field_hi=("periodic", "periodic", "pec"),
         nox=3, use_filter=True, cfl=1.0, moving_window_dir=2, moving_window_v=1.0, max_step=max_step,
