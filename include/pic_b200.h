@@ -611,6 +611,37 @@ int pic_deposit_charge(const pic_soa* p, long offset, long np, const pic_fab* rh
                        const double xyzmin[3], const int lo[3], double q, int nox, void* stream);
 int pic_apply_pec_rho(const pic_fab* rho, const pic_geom* g, const pic_boundaries* b, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Cold relativistic fluid species (WarpXFluidContainer, Source/Fluids/WarpXFluidContainer.cpp), 3D Cartesian,
+ * periodic domains, lab frame.  A fluid's state U is four all-nodal components {N, NUx, NUy, NUz} on the run's
+ * cell box with 2 guard nodes (AllocateLevelMFs :142-164).  Products and sums are rounded as the reference's
+ * CPU build rounds them (no multiply-add contraction).
+ * pic_fluid_gather_push:     GatherAndPush :967-1238 without external fields or boost: at the valid nodes with
+ *   N > 0, E and B interpolated to the node (ablastr::coarsen::sample::Interp), U pushed with Higuera-Cary,
+ *   N U written back.  E / B guards must be filled (one guard node).
+ * pic_fluid_advect:          AdvectivePush_Muscl :421-893 from U_in into U_out (valid nodes only; two arrays:
+ *   one fused kernel reads neighbours while others are written).  The 2 guard nodes of U_in must be filled
+ *   (the FillBoundary of ApplyBcFluidsAndComms :413-417).  counters: NULL, or 2 device words that count the
+ *   nodes whose edges are zero (N <= 0) and the directions the positivity limiter reset.
+ * pic_fluid_deposit_current: DepositCurrent :1276-1398: J += the Yee-point average of q N U / gamma of the
+ *   two (or one) nodes it lies between, at the points this box owns (every index in [box_lo, box_hi]: each
+ *   point shared by bricks or periodic images is added once; J's SumBoundary completes the copies).
+ * pic_fluid_deposit_charge:  DepositCharge :1240-1273: rho += q N at the owned nodes.  rho: nodal, same box. */
+int pic_fluid_gather_push(const pic_fab U[4], const pic_fab E[3], const pic_fab B[3], double q, double m,
+                          double dt, void* stream);
+int pic_fluid_advect(const pic_fab U_in[4], const pic_fab U_out[4], const double dx[3], double dt,
+                     unsigned long long* counters, void* stream);
+int pic_fluid_deposit_current(const pic_fab U[4], const pic_fab J[3], double q, void* stream);
+int pic_fluid_deposit_charge(const pic_fab* N, const pic_fab* rho, double q, void* stream);
+/* The C++ driver's fluid species (fluids.species_names): pic_engine_evolve runs WarpXFluidContainer::Evolve
+ * (:257-314) for every fluid after the particle species' push and deposit (myfl->Evolve, Source/Evolve/
+ * WarpXEvolve.cpp:1171-1178): gather + push, FillBoundary of N and NU, advection into the other state, current deposit.
+ * stateA: the initial state on the engine's box (2 guard nodes), stateB: a second state of the same shape; both are
+ * borrowed.  One rank, periodic faces, no moving window, no boost, no particle species or antennas; refused calls
+ * leave the engine unchanged.  pic_engine_fluid_state: which state of fluid i is current (0 = A, 1 = B), -1 if none. */
+int pic_engine_add_fluid_species(void* h, double q, double m, const pic_fab stateA[4], const pic_fab stateB[4]);
+int pic_engine_fluid_state(void* h, int i);
+
 /* Number of kernels launched by this library since load (bench.py's gpu_launches). */
 long pic_launch_count(void);
 

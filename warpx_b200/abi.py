@@ -175,6 +175,18 @@ def LWFA_SIGNATURES(fabp, soap, gp, bp, lp, jp, dp, ip, vp):
     }
 
 
+def FLUID_SIGNATURES(fabp, dp, vp):
+    """ctypes signatures of the fluid-species entry points of include/pic_b200.h (a fluid state is 4 pic_fab)."""
+    return {
+        "pic_fluid_gather_push": (C.c_int, [fabp, fabp, fabp, C.c_double, C.c_double, C.c_double, vp]),
+        "pic_fluid_advect": (C.c_int, [fabp, fabp, dp, C.c_double, vp, vp]),
+        "pic_fluid_deposit_current": (C.c_int, [fabp, fabp, C.c_double, vp]),
+        "pic_fluid_deposit_charge": (C.c_int, [fabp, fabp, C.c_double, vp]),
+        "pic_engine_add_fluid_species": (C.c_int, [vp, C.c_double, C.c_double, fabp, fabp]),
+        "pic_engine_fluid_state": (C.c_int, [vp, C.c_int]),
+    }
+
+
 SOLVER_YEE, SOLVER_CKC = 0, 1
 PIC_ERR_ABORT, PIC_ERR_RETURN = 0, 1
 PUSHER_BORIS, PUSHER_VAY, PUSHER_HC = 0, 1, 2

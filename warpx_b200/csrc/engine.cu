@@ -73,9 +73,18 @@ struct Laser {
 // Per-stage CUDA-event timing of the step driver (pic_engine_enable_timing / pic_engine_stage_ms): the events are
 // recorded on the stream the stages are launched on, inside the same pic_engine_evolve calls a benchmark times.
 enum { ST_FILL_EB = 0, ST_GATHER_PUSH, ST_ZERO_J, ST_DEPOSIT, ST_SYNC_J, ST_EVOLVE_B, ST_FILL_B, ST_EVOLVE_E, ST_FILL_E,
-       ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_COUNT };
+       ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_FLUID, ST_COUNT };
 static const char* const stage_names[ST_COUNT] = {"fill_boundary_eb", "gather_push", "zero_j", "deposit", "sync_current",
-    "evolve_b", "fill_boundary_b", "evolve_e", "fill_boundary_e", "wrap", "migrate", "sort", "nci_filter", "move_window", "push_p", "filter_j"};
+    "evolve_b", "fill_boundary_b", "evolve_e", "fill_boundary_e", "wrap", "migrate", "sort", "nci_filter", "move_window", "push_p", "filter_j",
+    "fluid"};
+// Cold fluid species (WarpXFluidContainer): two borrowed states of N, NUx, NUy, NUz; the advection writes one from the
+// other and `cur` names the current one.
+struct Fluid {
+    double q, m;
+    pic_fab U[2][4];
+    int cur = 0;
+};
+
 struct StageRec { int st; cudaEvent_t a, b; };
 struct Timing {
     bool on = false;
@@ -128,6 +137,7 @@ struct Engine {
     size_t shift_tmp_bytes = 0;
     int* host_count = nullptr;                   // pinned host int (particles lost per boundary pass)
     std::vector<Laser> lasers;
+    std::vector<Fluid> fluids;
 };
 
 struct Stage {      // records the events of one stage when timing is on
@@ -652,6 +662,18 @@ static int apply_particle_boundaries(Engine& e, void* stream) {
     return 0;
 }
 
+// WarpXFluidContainer::Evolve (Source/Fluids/WarpXFluidContainer.cpp:257-314) on a periodic domain: GatherAndPush,
+// the FillBoundary of N and NU with all 2 guard nodes (ApplyBcFluidsAndComms :413-417), AdvectivePush_Muscl into the
+// other state, DepositCurrent into the J the particles deposit into (filtered afterwards like theirs).
+static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
+    pic_fab* U = fl.U[fl.cur];
+    ENG_CALL(pic_fluid_gather_push(U, &e.fab[0], &e.fab[3], fl.q, fl.m, e.dt, s));
+    for (int d = 0; d < 3; ++d) ENG_CALL(halo_sweep(e, U, 4, d, 2, 0, s));
+    ENG_CALL(pic_fluid_advect(U, fl.U[1 - fl.cur], e.dx, e.dt, nullptr, s));
+    fl.cur = 1 - fl.cur;
+    return pic_fluid_deposit_current(fl.U[fl.cur], e.use_filter ? e.jdep : &e.fab[6], fl.q, s);
+}
+
 static int one_step(Engine& e, bool last, void* s) {
     // ---- ExplicitFillBoundaryEBUpdateAux ----
     if (e.is_synchronized) {
@@ -664,6 +686,7 @@ static int one_step(Engine& e, bool last, void* s) {
     }
     // ---- OneStep_nosub ----
     ENG_CALL(push_particles_and_deposit(e, s));
+    for (auto& fl : e.fluids) { Stage t(e, ST_FLUID, s); ENG_CALL(evolve_fluid(e, fl, s)); }   // myfl->Evolve, :1171-1178
     if (e.use_filter) { Stage t(e, ST_FILTER, s); ENG_CALL(pic_apply_filter_multi(e.jdep, &e.fab[6], 3, e.npass, s)); }
     { Stage t(e, ST_SYNC_J, s); ENG_CALL(sync_current(e, s)); }
     { Stage t(e, ST_EVOLVE_B, s); ENG_CALL(evolve_b(e, 0.5 * e.dt, s)); }
@@ -815,6 +838,7 @@ extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa
                                       void* stream) {
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(capacity >= bufA->np, "pic_engine_add_species: capacity %ld < np %ld", capacity, (long)bufA->np);
+    PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_species: runs with fluid species take no particle species yet");
     Species sp;
     sp.capacity = capacity;
     sp.q = q; sp.m = m; sp.buf[0] = *bufA; sp.buf[1] = *bufB; sp.cur = 0; sp.has_bins = false; sp.sort_work = sort_work;
@@ -1026,6 +1050,7 @@ extern "C" int pic_engine_set_injector(void* h, int isp, const pic_plasma_inject
 }
 extern "C" int pic_engine_add_laser(void* h, const pic_laser_antenna* prm, const pic_soa* p, long capacity) {
     Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_laser: runs with fluid species take no antennas yet");
     double info[4];
     PIC_REQUIRE(same_boost(*e, prm->gamma_boost, prm->beta_boost), "pic_engine_add_laser: the antenna's gamma_boost / beta_boost differ from pic_engine_set_boost");
     ENG_CALL(pic_laser_antenna_info(prm, e->dx, info));
@@ -1062,4 +1087,37 @@ extern "C" int pic_engine_evolve(void* h, int numsteps, int synchronize_last, vo
     Engine* e = static_cast<Engine*>(h);
     for (int n = 0; n < numsteps; ++n) ENG_CALL(one_step(*e, synchronize_last && n == numsteps - 1, stream));
     return 0;
+}
+
+// A cold fluid species (fluids.species_names): stateA holds the initial N, NUx, NUy, NUz on this engine's box with 2
+// guard nodes, stateB is a second state of the same shape (borrowed; the driver advects from one into the other, see
+// pic_engine_fluid_state).  One rank, periodic faces, no moving window, no boost, no particle species or antennas.
+// Every precondition is checked before the engine is changed.
+extern "C" int pic_engine_add_fluid_species(void* h, double q, double m, const pic_fab stateA[4], const pic_fab stateB[4]) {
+    Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e && stateA && stateB, "pic_engine_add_fluid_species: null argument");
+    PIC_REQUIRE(e->all_periodic, "pic_engine_add_fluid_species: every face must be periodic");
+    PIC_REQUIRE(!e->do_moving_window, "pic_engine_add_fluid_species: moving windows are not supported");
+    PIC_REQUIRE(e->gamma_boost == 1.0, "pic_engine_add_fluid_species: boosted frames are not supported");
+    PIC_REQUIRE(e->comm == nullptr, "pic_engine_add_fluid_species: one rank only");
+    PIC_REQUIRE(e->species.empty() && e->lasers.empty(), "pic_engine_add_fluid_species: runs with particle species or antennas take no fluids yet");
+    PIC_REQUIRE(m > 0.0, "pic_engine_add_fluid_species: mass must be positive");
+    for (int b = 0; b < 2; ++b)
+        for (int c = 0; c < 4; ++c) {
+            const pic_fab& f = (b ? stateB : stateA)[c];
+            PIC_REQUIRE(f.p != nullptr, "pic_engine_add_fluid_species: component %d of state %d has no data", c, b);
+            for (int d = 0; d < 3; ++d)
+                PIC_REQUIRE(f.stag[d] == 1 && f.ng[d] == 2 && vlo(f, d) == e->box_lo[d] && vhi(f, d) == e->box_hi[d] + 1,
+                            "pic_engine_add_fluid_species: a state is 4 all-nodal components on the engine's box with 2 guard nodes");
+        }
+    Fluid fl;
+    fl.q = q; fl.m = m;
+    for (int c = 0; c < 4; ++c) { fl.U[0][c] = stateA[c]; fl.U[1][c] = stateB[c]; }
+    e->fluids.push_back(fl);
+    return 0;
+}
+// Which of the two states of fluid i is current (0: stateA, 1: stateB); -1 if there is no such fluid.
+extern "C" int pic_engine_fluid_state(void* h, int i) {
+    Engine* e = static_cast<Engine*>(h);
+    return (i >= 0 && i < (int)e->fluids.size()) ? e->fluids[i].cur : -1;
 }

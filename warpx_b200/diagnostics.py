@@ -189,6 +189,8 @@ def write_checkpoint(sim, prefix, iteration=None, file_min_digits=5):
     from . import parallel
     if sim.moving_window is not None:
         raise NotImplementedError("checkpoints of moving-window runs (the window position is not restored yet)")
+    if getattr(sim, "fluids", None):
+        raise NotImplementedError("checkpoints of runs with fluid species (the fluid state is not written yet)")
     it = sim.istep if iteration is None else int(iteration)
     root = "%s%0*d" % (prefix, file_min_digits, it)
     lev = os.path.join(root, "Level_0")

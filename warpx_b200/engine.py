@@ -243,6 +243,32 @@ class Species:
         return self.buf[self.cur][self.NAMES.index(name), :self.np]
 
 
+class FluidSpecies:
+    """A cold relativistic fluid (WarpXFluidContainer): two states of four all-nodal components N, NUx, NUy, NUz
+    with 2 guard nodes; the advection writes one from the other, `cur` names the current one."""
+    NAMES = ("N", "NUx", "NUy", "NUz")
+    NG = (2, 2, 2)
+
+    def __init__(self, sim, name, q, m):
+        t = sim.torch
+        self.name, self.q, self.m = name, float(q), float(m)
+        self.data, self.fabs = [], []
+        for _ in range(2):
+            descs, arrs = [], []
+            for _c in range(4):
+                d = abi.make_fab(None, sim.box_lo, sim.box_hi, self.NG, (1, 1, 1))
+                a = t.zeros(d.shape, dtype=t.float64, device=sim.device)
+                d.p = a.data_ptr()
+                descs.append(d)
+                arrs.append(a)
+            self.data.append(arrs)
+            self.fabs.append((abi.pic_fab * 4)(*descs))
+        self.cur = 0
+
+    def state(self, which=None):
+        return self.fabs[self.cur if which is None else which]
+
+
 class Simulation:
     def __init__(self, n_cell, prob_lo, prob_hi, nox, galerkin=1, pusher=abi.PUSHER_BORIS,
                  solver=abi.SOLVER_YEE, cfl=1.0, dt=None, dist=None, sort_interval=4,
@@ -312,6 +338,7 @@ class Simulation:
         self.J = (abi.pic_fab * 3)(*descs[6:9])
         self.halo = parallel.HaloExchanger(self.dec, _DeviceOps(self), dist)
         self.species = []
+        self.fluids = []
         self.is_synchronized = True
         self.istep = 0
         self._scratch = t.zeros(8, dtype=t.float64, device=self.device)
@@ -414,6 +441,8 @@ class Simulation:
         (default: rank << 40 | index)."""
         if capacity_factor is None:
             capacity_factor = 1.0 if self.world == 1 else 1.25
+        if self.fluids:
+            raise NotImplementedError("runs with fluid species take no particle species")
         arrays = dict(x=x, y=y, z=z, w=w, ux=ux, uy=uy, uz=uz)
         cap = int(len(x) * capacity_factor) + (0 if self.world == 1 else 65536)
         sp = Species(self, name, q, m, arrays, cap, ids=ids)
@@ -496,6 +525,42 @@ class Simulation:
                                             self.stream))
         self._sync_from_native()
         return sp
+
+    def add_fluid_species(self, name, q, m, density, momentum):
+        """fluids.species_names / <species>.*: a cold relativistic fluid (WarpXFluidContainer), initialised like InitData
+        (Source/Fluids/WarpXFluidContainer.cpp:166-254) in the lab frame over this rank's valid nodes, at
+        x = prob_lo + i dx: N = n, NU = n u c.  density(x, y, z) -> n [m^-3] and momentum(x, y, z) -> (ux, uy, uz) in
+        units of c are evaluated here on the host in float64, on numpy arrays of node coordinates.  One rank, periodic
+        domains without a moving window or boost, no particle species or antennas (the fluid runs in the C++ driver or
+        in the Python sequencer); other runs are refused before anything is allocated."""
+        if self.nonperiodic:
+            raise NotImplementedError("fluid species: every face must be periodic")
+        if self.moving_window is not None:
+            raise NotImplementedError("fluid species: moving windows are not supported")
+        if self.gamma_boost > 1.0:
+            raise NotImplementedError("fluid species: boosted frames are not supported")
+        if self.world > 1:
+            raise NotImplementedError("fluid species: one rank only")
+        if self.species or self.lasers:
+            raise NotImplementedError("fluid species: runs with particle species or antennas are not supported")
+        coords = [self.prob_lo[d] + np.arange(self.box_lo[d], self.box_hi[d] + 2) * self.dx[d] for d in range(3)]
+        Z, Y, X = np.meshgrid(coords[2], coords[1], coords[0], indexing="ij")
+        n = np.broadcast_to(np.asarray(density(X, Y, Z), dtype=np.float64), X.shape)
+        u = [np.broadcast_to(np.asarray(v, dtype=np.float64), X.shape) for v in momentum(X, Y, Z)]
+        fl = FluidSpecies(self, name, q, m)
+        vs = fl.fabs[0][0].valid_slices()
+        vals = (n, n * (u[0] * C_LIGHT), n * (u[1] * C_LIGHT), n * (u[2] * C_LIGHT))
+        for c in range(4):
+            fl.data[0][c][vs].copy_(self.torch.from_numpy(np.array(vals[c], dtype=np.float64)))
+        if self.native:
+            check(self.L.pic_engine_add_fluid_species(self.native, fl.q, fl.m, fl.fabs[0], fl.fabs[1]))
+        self.fluids.append(fl)
+        return fl
+
+    def fluid_numpy(self, i):
+        """(descriptor, {"N", "NUx", "NUy", "NUz": numpy array [k, j, i], guards included}) of fluid species i."""
+        fl = self.fluids[i]
+        return fl.state()[0], {name: fl.data[fl.cur][c].cpu().numpy() for c, name in enumerate(FluidSpecies.NAMES)}
 
     def add_laser(self, laser):
         """lasers.names / <laser>.*: a Gaussian antenna (LaserParticleContainer ctor + InitData,
@@ -633,6 +698,21 @@ class Simulation:
         for sp in self.species:
             self._timed("gather_push", self.PushPX, sp, self.dt)
             self._timed("deposit", self.DepositCurrent, sp, self.dt, -0.5 * self.dt)  # relative_time, PhysicalParticleContainer.cpp:2029
+        for fl in self.fluids:                               # myfl->Evolve, WarpXEvolve.cpp:1171-1178
+            self.EvolveFluid(fl)
+
+    def EvolveFluid(self, fl):
+        """WarpXFluidContainer::Evolve (Source/Fluids/WarpXFluidContainer.cpp:257-314) on a periodic domain: GatherAndPush,
+        the FillBoundary of N and NU (ApplyBcFluidsAndComms :413-417), AdvectivePush_Muscl into the other state,
+        DepositCurrent into J."""
+        L, st = self.L, self.stream
+        self._timed("fluid_gather_push", lambda: check(L.pic_fluid_gather_push(fl.state(), self.E, self.B, fl.q, fl.m,
+                                                                                 self.dt, st)))
+        self._timed("fluid_fill_boundary", self.halo.fill_boundary, list(fl.state()), list(FluidSpecies.NG))
+        self._timed("fluid_advect", lambda: check(L.pic_fluid_advect(fl.state(), fl.state(1 - fl.cur), abi.dbl3(self.dx),
+                                                                       self.dt, None, st)))
+        fl.cur = 1 - fl.cur
+        self._timed("fluid_deposit", lambda: check(L.pic_fluid_deposit_current(fl.state(), self.J, fl.q, st)))
 
     def SortParticlesByBin(self, sp):
         bins = abi.pic_bins()
@@ -745,6 +825,8 @@ class Simulation:
             self.istep += numsteps
             self.is_synchronized = bool(synchronize_last)
             self._sync_from_native()
+            for i, fl in enumerate(self.fluids):
+                fl.cur = self.L.pic_engine_fluid_state(self.native, i)
             # the moving window translates the problem domain; t_new
             dom = (C.c_double * 6)()
             self.L.pic_engine_prob_domain(self.native, dom)
@@ -832,6 +914,8 @@ class Simulation:
             if self.nonperiodic:
                 check(self.L.pic_apply_pec_rho(C.byref(one_d), C.byref(self.geom), C.byref(self.boundaries), self.stream))
             rho += one
+        for fl in self.fluids:                                             # RhoFunctor.cpp:47-51
+            check(self.L.pic_fluid_deposit_charge(C.byref(fl.state()[0]), C.byref(rho_d), fl.q, self.stream))
         work_d, work, ngw = rho_d, rho, [ng] * 3
         if self.use_filter:
             ngw = [ng + self.filter_npass[d] for d in range(3)]

@@ -126,6 +126,7 @@ def bind(L):
         "pic_engine_prob_domain": (None, [vp, dp]),
     }
     sig.update(abi.LWFA_SIGNATURES(fabp, soap, gp, bndp, lasp, injp, dp, ip, vp))
+    sig.update(abi.FLUID_SIGNATURES(fabp, dp, vp))
     for name, (res, args) in sig.items():
         fn = getattr(L, name)      # AttributeError if include/pic_b200.h and the library disagree
         fn.restype = res

@@ -72,6 +72,29 @@ def langmuir_3d(n=64, ppc=(1, 1, 1), lx=40.0e-6, n0=2.0e24, epsilon=0.01):
                 analytic=dict(k=k, wp=wp, epsilon=epsilon))
 
 
+def langmuir_fluid_3d(n=64, lx=40.0e-6, n0=2.0e24, epsilon=0.01):
+    """Examples/Tests/langmuir_fluids/inputs_test_3d_langmuir_fluid: electron and positron cold fluids of density n0
+    with the Langmuir wave's momenta, periodic, Yee, cfl 1, 40 steps.  Each fluid: name, q, m, density(x, y, z) and
+    momentum(x, y, z) -> (ux, uy, uz) in units of c, for Simulation.add_fluid_species."""
+    wp = np.sqrt(2.0 * n0 * Q_E ** 2 / (EP0 * M_E))   # the deck's my_constants
+    kp = wp / C
+    k = 2.0 * 2.0 * np.pi / lx
+    a = epsilon * k / kp
+
+    def density(x, y, z):
+        return np.full(np.shape(x), n0)
+
+    def momentum(sign):
+        return lambda x, y, z: (sign * a * np.sin(k * x) * np.cos(k * y) * np.cos(k * z),
+                                sign * a * np.cos(k * x) * np.sin(k * y) * np.cos(k * z),
+                                sign * a * np.cos(k * x) * np.cos(k * y) * np.sin(k * z))
+
+    fluids = [dict(name="electrons", q=-Q_E, m=M_E, density=density, momentum=momentum(1.0)),
+              dict(name="positrons", q=Q_E, m=M_E, density=density, momentum=momentum(-1.0))]
+    return dict(n_cell=(n, n, n), prob_lo=(-lx / 2,) * 3, prob_hi=(lx / 2,) * 3, fluids=fluids, max_step=40,
+                analytic=dict(k=k, wp=np.sqrt(2.0 * n0 * Q_E ** 2 / (EP0 * M_E)), epsilon=epsilon))
+
+
 def philox_normal(seed, first_id, count, ncomp=3):
     """Counter-based N(0,1) numbers: particle `id` always gets the same values, independent of how
     the domain is decomposed (SURVEY.md section 8d, config 2).  numpy Philox4x64 keyed by `seed`,
