@@ -103,84 +103,6 @@ def lower_corner(prob_lo, dx, box_lo, ng):
     return [prob_lo[d] + dx[d] * lo[d] for d in range(3)], lo
 
 
-class NumpyHaloOps:
-    """CPU stand-in for the CUDA guard-cell kernels (same slab definitions as
-    warpx_b200/csrc/halo.cu) so that parallel.HaloExchanger can be exercised over gloo."""
-
-    def __init__(self, torch, n_cell):
-        self.torch, self.n_cell = torch, n_cell
-
-    def empty(self, n):
-        return self.torch.empty(n, dtype=self.torch.float64)
-
-    @staticmethod
-    def _view(fab):
-        return fab.host      # numpy array [k, j, i] attached to the descriptor by the test
-
-    @staticmethod
-    def _range(fab, dim, side, ng, mode, unpack):
-        lc = fab.lo[dim] + fab.ng[dim]
-        hc = fab.hi[dim] - fab.ng[dim] - fab.stag[dim]
-        st = fab.stag[dim]
-        if mode == 0:
-            count = ng
-            first = (hc + 1 - ng if side else lc + st) if not unpack else (hc + 1 + st if side else lc - ng)
-        else:
-            count = ng + st
-            first = (hc + 1 if side else lc - ng) if not unpack else (hc + 1 - ng if side else lc)
-        return first - fab.lo[dim], count
-
-    def slab_count(self, fab, dim, ng, mode):
-        n = 1
-        for d in range(3):
-            if d != dim:
-                n *= fab.hi[d] - fab.lo[d] + 1
-        return n * (ng if mode == 0 else ng + fab.stag[dim])
-
-    def _slice(self, fab, dim, first, count):
-        sl = [slice(None)] * 3
-        sl[2 - dim] = slice(first, first + count)
-        return tuple(sl)
-
-    def pack(self, fab, dim, side, ng, mode, buf):
-        first, count = self._range(fab, dim, side, ng, mode, False)
-        a = self._view(fab)[self._slice(fab, dim, first, count)]
-        buf.copy_(self.torch.from_numpy(np.ascontiguousarray(a).ravel()))
-
-    def unpack(self, fab, dim, side, ng, mode, buf):
-        first, count = self._range(fab, dim, side, ng, mode, True)
-        sl = self._slice(fab, dim, first, count)
-        a = self._view(fab)
-        v = buf.numpy().reshape(a[sl].shape)
-        if mode:
-            a[sl] += v
-        else:
-            a[sl] = v
-
-    def fill_local(self, fab, dim, ng):
-        a = self._view(fab)
-        N = self.n_cell[dim]
-        vl, vh = fab.ng[dim], fab.hi[dim] - fab.lo[dim] - fab.ng[dim]
-        ax = 2 - dim
-        idx = np.arange(a.shape[ax])
-        lo_g, hi_g = idx[vl - ng:vl], idx[vh + 1:vh + 1 + ng]
-        a_sw = np.moveaxis(a, ax, 0)
-        a_sw[lo_g] = a_sw[lo_g + N]
-        a_sw[hi_g] = a_sw[hi_g - N]
-
-    def sum_local(self, fab, dim, ng):
-        a = np.moveaxis(self._view(fab), 2 - dim, 0)
-        N = self.n_cell[dim]
-        vl, vh = fab.ng[dim], fab.hi[dim] - fab.lo[dim] - fab.ng[dim]
-        if fab.stag[dim]:
-            s = a[vl] + a[vh]
-            a[vl] = s
-            a[vh] = s
-        for g in range(1, ng + 1):
-            a[vl - g + N] += a[vl - g]
-            a[vh + g - N] += a[vh + g]
-
-
 # ---------------------------------------------------------------------------------------------
 # Outputs of the oracle's leaf arithmetic and stages on fixed, seeded inputs.  tests/golden/make_reference_leaves.py
 # records them with the reference's own headers compiled in (oracle/_ref) as SHA-256 digests in

@@ -89,12 +89,10 @@ def main():
                                        box_lo=dec3.box_lo, box_hi=dec3.box_hi)
     s = mine["species"][0]
     so = wl["species"][0]
-    # warpx.use_filter = 0 / 1 (bilinear, 1 pass); C++ driver over its own NCCL communicator, and the
-    # Python sequencer over torch.distributed as the cross-check
-    for filt, native in ((False, True), (True, True), (False, False)) if "order3" in sections else ():
+    # warpx.use_filter = 0 / 1 (bilinear, 1 pass); C++ driver over its own NCCL communicator
+    for filt in (False, True) if "order3" in sections else ():
         sim3 = Simulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=3, dist=dist, sort_interval=4,
-                          use_filter=filt, native_driver=native)
-        assert bool(sim3.native) == native
+                          use_filter=filt)
         sim3.add_species(s["name"], s["q"], s["m"], s["x"], s["y"], s["z"], s["w"], s["ux"], s["uy"], s["uz"])
         sim3.Evolve(12)
         e, b = sim3.field_energy()
@@ -106,7 +104,7 @@ def main():
             eo, bo = osim.field_energy()
             good = abs(e - eo) <= 1e-10 * eo and abs(b - bo) <= 1e-8 * bo and npart == len(so["x"])
             ok &= good
-            print(f"[order3 x{world} filter={int(filt)} native={int(native)}] field energy E {e:.12e} vs oracle {eo:.12e}; "
+            print(f"[order3 x{world} filter={int(filt)}] field energy E {e:.12e} vs oracle {eo:.12e}; "
                   f"B {b:.12e} vs {bo:.12e}; particles {npart}: {'ok' if good else 'FAIL'}")
         sim3.close()
         del sim3

@@ -1,6 +1,6 @@
 """CPU tests (-m "not gpu") of the cold relativistic fluid species: the numpy restatement (tests/fluid_oracle.py)
 against WarpX's regression checksums of test_3d_langmuir_fluid and against known answers, and the product's fluid
-kernels and Python sequencer, built for the host by tests/host_harness, against that restatement."""
+kernels and C++ step driver, built for the host by tests/host_harness, against that restatement."""
 import ctypes as C
 import json
 import os
@@ -115,7 +115,7 @@ def test_vacuum_edge_keeps_density_non_negative_and_exercises_both_paths(orc):
     assert run.counters["zero_edges"] > 0 and run.counters["limited"] > 0, run.counters
 
 
-# ---- the product's kernels and sequencer, built for the host ------------------------------------------------------
+# ---- the product's kernels and step driver, built for the host ---------------------------------------------------
 @pytest.fixture(scope="module")
 def host():
     import torch
@@ -141,13 +141,12 @@ def test_host_fluid_advection_matches_the_reference_headers(host):
     fluid_cases.check_reference_fixture(L, torch, torch.device("cpu"))
 
 
-@pytest.mark.parametrize("native", [True, False])
-def test_host_fluid_loop_matches_oracle(orc, native):
-    """The C++ driver (native) and the Python sequencer with two fluids run the same stages at the same place of the
-    step as the oracle loop.  The fluid stages agree bit for bit; the field solver's kernels and the oracle's round a
-    few sums in another order, so fields and fluids are compared to 1e-12 of their scale."""
+def test_host_fluid_loop_matches_oracle(orc):
+    """The C++ driver with two fluids runs the same stages at the same place of the step as the oracle loop.  The
+    fluid stages agree bit for bit; the field solver's kernels and the oracle's round a few sums in another order, so
+    fields and fluids are compared to 1e-12 of their scale."""
     from fluid_cases import rel_linf
-    sim, run = _host_pair(orc, native, 4)
+    sim, run = _host_pair(orc, 4)
     for c in range(9):
         d, a = sim.field_numpy(c)
         V = d.valid_slices()
@@ -162,31 +161,18 @@ def test_host_fluid_loop_matches_oracle(orc, native):
     assert rel_linf(rho[r.desc.valid_slices()], r.a[r.desc.valid_slices()]) <= 1e-12
 
 
-def _host_pair(orc, native, steps):
+def _host_pair(orc, steps):
     from host_harness import harness
     Sim = harness.host_simulation_class()
     wl = workloads.langmuir_fluid_3d(n=12)
-    sim = Sim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=1, native_driver=native)
-    run = fo.FluidRun(orc, wl["n_cell"], wl["prob_lo"], wl["prob_hi"]) if orc else None
+    sim = Sim(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=1)
+    run = fo.FluidRun(orc, wl["n_cell"], wl["prob_lo"], wl["prob_hi"])
     for f in wl["fluids"]:
         sim.add_fluid_species(f["name"], f["q"], f["m"], f["density"], f["momentum"])
-        if run:
-            run.add_fluid(f["q"], f["m"], f["density"], f["momentum"])
+        run.add_fluid(f["q"], f["m"], f["density"], f["momentum"])
     sim.Evolve(steps)
-    if run:
-        run.evolve(steps)
+    run.evolve(steps)
     return sim, run
-
-
-def test_host_driver_matches_sequencer_bit_for_bit():
-    a, _ = _host_pair(None, True, 5)
-    b, _ = _host_pair(None, False, 5)
-    for c in range(9):
-        assert np.array_equal(a.field_numpy(c)[1], b.field_numpy(c)[1]), c
-    for i in range(2):
-        for name in ("N", "NUx", "NUy", "NUz"):
-            V = a.fluid_numpy(i)[0].valid_slices()
-            assert np.array_equal(a.fluid_numpy(i)[1][name][V], b.fluid_numpy(i)[1][name][V]), (i, name)
 
 
 def _fabs(desc, fill, n=4):
@@ -218,14 +204,13 @@ def test_host_fluid_refusals_leave_the_run_untouched():
         with pytest.raises(NotImplementedError, match=msg):
             sim.add_fluid_species(*args)
         assert sim.fluids == []
-    for native in (True, False):
-        sim = Sim(*dom, nox=1, native_driver=native)
-        sim.add_fluid_species(*args)
-        with pytest.raises(NotImplementedError, match="fluid"):
-            sim.add_species(p["name"], p["q"], p["m"], p["x"], p["y"], p["z"], p["w"], p["ux"], p["uy"], p["uz"])
-        assert sim.species == []
-        with pytest.raises(NotImplementedError, match="fluid"):
-            diagnostics.write_checkpoint(sim, "/nonexistent/chk")
+    sim = Sim(*dom, nox=1)
+    sim.add_fluid_species(*args)
+    with pytest.raises(NotImplementedError, match="fluid"):
+        sim.add_species(p["name"], p["q"], p["m"], p["x"], p["y"], p["z"], p["w"], p["ux"], p["uy"], p["uz"])
+    assert sim.species == []
+    with pytest.raises(NotImplementedError, match="fluid"):
+        diagnostics.write_checkpoint(sim, "/nonexistent/chk")
     # the library refuses bad arguments before it changes anything
     L = harness.host_library()
     good = abi.make_fab(None, (0, 0, 0), (7, 7, 7), (2, 2, 2), (1, 1, 1))

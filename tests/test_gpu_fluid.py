@@ -1,5 +1,5 @@
 """GPU tests of the cold relativistic fluid species: each kernel against the numpy restatement (tests/fluid_oracle.py),
-and the Langmuir fluid deck through the Python sequencer against WarpX's regression checksums and the oracle loop."""
+and the Langmuir fluid deck through the C++ driver against WarpX's regression checksums and the oracle loop."""
 import json
 import os
 
@@ -50,24 +50,23 @@ def deck_oracle(orc):
     return run
 
 
-def _deck(native):
+def _deck():
     from warpx_b200.engine import Simulation
     wl = workloads.langmuir_fluid_3d()
-    sim = Simulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=1, native_driver=native)
+    sim = Simulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=1)
     for f in wl["fluids"]:
         sim.add_fluid_species(f["name"], f["q"], f["m"], f["density"], f["momentum"])
     sim.Evolve(wl["max_step"])
     return sim
 
 
-@pytest.mark.parametrize("native", [True, False])
-def test_langmuir_fluid_deck_golden_checksums_and_oracle(cuda, deck_oracle, native):
-    """inputs_test_3d_langmuir_fluid, 40 steps, on the device through the C++ driver (native) or the Python sequencer:
-    WarpX's checksums at rtol 1e-9, and the oracle loop's fields (1e-9 of each vector's scale), field energy (1e-10)
-    and fluid state (1e-9 of each component's scale)."""
+def test_langmuir_fluid_deck_golden_checksums_and_oracle(cuda, deck_oracle):
+    """inputs_test_3d_langmuir_fluid, 40 steps, on the device through the C++ driver: WarpX's checksums at rtol 1e-9,
+    and the oracle loop's fields (1e-9 of each vector's scale), field energy (1e-10) and fluid state (1e-9 of each
+    component's scale)."""
     with open(os.path.join(ROOT, "tests", "golden", "warpx_fluid_checksums.json")) as f:
         g = json.load(f)["test_3d_langmuir_fluid"]["lev=0"]
-    sim, run = _deck(native), deck_oracle
+    sim, run = _deck(), deck_oracle
     for c, name in enumerate(abi.COMP_NAMES):
         d, a = sim.field_numpy(c)
         v = _cell_centre_checksum(d, a)
@@ -89,17 +88,6 @@ def test_langmuir_fluid_deck_golden_checksums_and_oracle(cuda, deck_oracle, nati
         for c, name in enumerate(("N", "NUx", "NUy", "NUz")):
             ref = run.fluids[i]["state"][c][V]
             assert np.max(np.abs(st[name][V] - ref)) <= 1e-9 * np.max(np.abs(ref)), (i, name)
-
-
-def test_langmuir_fluid_deck_driver_matches_sequencer(cuda):
-    """The C++ driver and the Python sequencer launch the same kernels in the same order: identical bits."""
-    a, b = _deck(True), _deck(False)
-    for c in range(9):
-        assert np.array_equal(a.field_numpy(c)[1], b.field_numpy(c)[1]), c
-    for i in range(2):
-        V = a.fluid_numpy(i)[0].valid_slices()
-        for name in ("N", "NUx", "NUy", "NUz"):
-            assert np.array_equal(a.fluid_numpy(i)[1][name][V], b.fluid_numpy(i)[1][name][V]), (i, name)
 
 
 def test_fluid_refusals_on_the_device(cuda):

@@ -109,7 +109,7 @@ MODE_CASES = ([DEFAULT] + [("deposit", m) for m in DEPOSIT_MODES if m != abi.PIC
 def test_gauss_in_every_mode(cuda, kind, mode):
     """128^3 at the benchmark's cell size, the benchmark's checkpoints, one mode switched at a time.  default:
     PIC_DEPOSIT_RUNS, pic_set_fdtd_mode(1) (EvolveB staged) and the tile gather.  deposit: every entry of
-    DEPOSIT_MODES (global = bins NULL, the Python step sequence).  fdtd 0: plain loads; fdtd 3: EvolveE staged as well.
+    DEPOSIT_MODES (global = use_bins=False: the C++ driver without bins).  fdtd 0: plain loads; fdtd 3: EvolveE staged as well.
     gather: pair mode 1."""
     from warpx_b200.lib import lib as piclib
     L = piclib()
@@ -168,15 +168,13 @@ def test_device_rho_matches_oracle(orc, cuda):
     sim.close()
 
 
-@pytest.mark.parametrize("native", [True, False])
-def test_gauss_check_sees_one_edited_weight(cuda, native):
+def test_gauss_check_sees_one_edited_weight(cuda):
     """Negative control on the device: between two Evolve chunks one particle's weight grows by half in the species
     array the step driver works on.  Three steps later G is off by more than 1e-4 of max|rho^0/ep0| within the
     particle's stencil, and within the bar everywhere else."""
     t = cuda
     wl = bench_workload(ORDER_N)
-    sim = make_sim(wl, native_driver=native)
-    assert bool(sim.native) == native
+    sim = make_sim(wl)
     sp = sim.species[0]
     G0, rho0 = simulation_gauss(sim)
     sim.Evolve(5, synchronize_last=False)

@@ -520,16 +520,12 @@ def test_plotfile_golden_checksums(orc, cuda, golden, tmp_path):
     sim.close()
 
 
-@pytest.mark.parametrize("solver,pusher,native", [(abi.SOLVER_YEE, abi.PUSHER_BORIS, True),
-                                                  (abi.SOLVER_YEE, abi.PUSHER_BORIS, False),
-                                                  (abi.SOLVER_CKC, abi.PUSHER_VAY, True)])
-def test_order3_loop_matches_oracle(orc, cuda, solver, pusher, native):
+@pytest.mark.parametrize("solver,pusher", [(abi.SOLVER_YEE, abi.PUSHER_BORIS), (abi.SOLVER_CKC, abi.PUSHER_VAY)])
+def test_order3_loop_matches_oracle(orc, cuda, solver, pusher):
     """Config 2 / 3 physics (order-3 Esirkepov, 8 ppc, Yee or CKC) at 32^3, 10 steps, with a
     Langmuir perturbation on top of the thermal spread so that the fields are well above noise."""
     wl = workloads.uniform_plasma_3d(n=32, ppc=(2, 2, 2), u_th=0.01, lx=5e-6, perturbation=0.01)
-    # native: the library's C++ step driver (csrc/engine.cu); otherwise the Python sequencer
-    sim, osim = _run_both(orc, cuda, wl, 3, 10, solver=solver, pusher=pusher, sort_interval=4, native_driver=native)
-    assert bool(sim.native) == native
+    sim, osim = _run_both(orc, cuda, wl, 3, 10, solver=solver, pusher=pusher, sort_interval=4)
     for c in range(9):
         d, a = sim.field_numpy(c)
         _, oa = osim.fab(c)
@@ -578,14 +574,12 @@ def test_config2_at_benchmark_size_matches_oracle(orc, cuda, n, deposit_mode):
     sim.close()
 
 
-@pytest.mark.parametrize("native,npass", [(True, (1, 1, 1)), (False, (1, 1, 1)), (True, (2, 1, 3))])
-def test_filtered_loop_matches_oracle(orc, cuda, native, npass):
+@pytest.mark.parametrize("npass", [(1, 1, 1), (2, 1, 3)])
+def test_filtered_loop_matches_oracle(orc, cuda, npass):
     """warpx.use_filter = 1 (the reference's default): J gets npass more guard cells, the bilinear
     filter runs before SumBoundaryJ.  Same bar as the unfiltered order-3 loop."""
     wl = workloads.uniform_plasma_3d(n=32, ppc=(2, 2, 2), u_th=0.01, lx=5e-6, perturbation=0.01)
-    sim, osim = _run_both(orc, cuda, wl, 3, 10, sort_interval=4, native_driver=native, use_filter=True,
-                          filter_npass=npass)
-    assert bool(sim.native) == native
+    sim, osim = _run_both(orc, cuda, wl, 3, 10, sort_interval=4, use_filter=True, filter_npass=npass)
     assert sim.ng_J == osim.guards()["ng_J"] == [4 + v for v in npass]
     for c in range(9):
         d, a = sim.field_numpy(c)

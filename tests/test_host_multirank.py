@@ -238,6 +238,15 @@ def test_boosted_frame_z_slabs_match_oracle(orc, hh):
             assert np.max(np.abs(a - B[k])) / (10.0 * workloads.C) <= 1e-9, (isp, k)
 
 
+def test_brick_decomposition_neighbours():
+    assert parallel.brick_grid(1) == (1, 1, 1) and parallel.brick_grid(2) == (2, 1, 1)
+    assert parallel.brick_grid(4) == (2, 2, 1) and parallel.brick_grid(8) == (2, 2, 2)
+    dec = parallel.Decomposition((64, 64, 64), (2, 2, 2), 5)      # coord (1, 0, 1)
+    assert dec.coord == (1, 0, 1) and dec.box_lo == (32, 0, 32) and dec.box_hi == (63, 31, 63)
+    assert dec.neighbour(0, 1) == dec.neighbour(0, 0) == dec.rank_of((0, 0, 1))   # two bricks: same rank
+    assert dec.neighbour(1, 1) == dec.rank_of((1, 1, 1))
+
+
 @pytest.mark.parametrize("nb,periodic", [((2, 1, 1), (1, 1, 1)), ((2, 2, 2), (1, 1, 1)), ((1, 1, 2), (1, 1, 0))])
 def test_halo_copy_and_add_match_oracle(orc, hh, nb, periodic):
     """pic_halo_copy / pic_halo_add -- the one-call replacements of ablastr's FillBoundary / SumBoundary -- on random

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """A/B of the experimental kernel variants on the benchmark workload, in ONE process (the 256^3 x 8 ppc state is
 generated and uploaded once): for every deposition variant (pic_set_deposit_mode 0..7, 12) and gather variant
-(pic_set_gather_mode 0..2) the per-stage times of the step (CUDA events around every stage, Python sequencer)
-and the whole-step time of the C++ driver.  Not a bench value -- a ranking tool for a scarce GPU slot:
+(pic_set_gather_mode 0..2) the whole-step time and the per-stage times of the C++ driver (its CUDA events around
+every stage).  Not a bench value -- a ranking tool for a scarce GPU slot:
 
     python tools/ab_modes.py --cells 256 > ab_modes.json
 
@@ -49,8 +49,8 @@ def main():
             s[k] = wl["prob_lo"][d] + (cell + rng.uniform(0.0, 1.0, len(cell))) * dxd
     names = ("x", "y", "z", "w", "ux", "uy", "uz")
 
-    def make(native):
-        sim = Simulation((n, n, n), wl["prob_lo"], wl["prob_hi"], nox=3, sort_interval=4, native_driver=native)
+    def make():
+        sim = Simulation((n, n, n), wl["prob_lo"], wl["prob_hi"], nox=3, sort_interval=4)
         sim.add_species("electrons", s["q"], s["m"], *[torch.from_numpy(s[k]) for k in names])
         return sim
 
@@ -86,7 +86,7 @@ def main():
             for g in (int(v) for v in args.gather_modes.split(",")):
                 L.pic_set_deposit_mode(d)
                 L.pic_set_gather_mode(g)
-                sim = make(True)
+                sim = make()
                 sim.Evolve(4, synchronize_last=False)
                 sim.enable_stage_timing(True)
                 ms = timed(sim, args.steps)
@@ -105,7 +105,7 @@ def main():
              [(0, g) for g in (int(v) for v in args.gather_modes.split(",")) if g]
     out = {"cells": n, "ppc": args.ppc ** 3, "steps": args.steps, "variants": []}
     # whole step, C++ driver
-    sim = make(True)
+    sim = make()
     sim.Evolve(4, synchronize_last=False)
     for d, g in combos + [combos[0]]:                    # the default again at the end: drift of the state
         L.pic_set_deposit_mode(d)

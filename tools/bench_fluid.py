@@ -2,10 +2,10 @@
 
     python tools/bench_fluid.py [--n 256] [--steps 40] [--warmup 5]
 
-Per fluid stage: milliseconds per call from CUDA events over the timed steps (Simulation.enable_stage_timing), the
-algorithmic bytes per node the stage must move (computed here from the array shapes, fp64), the achieved rate and its
-fraction of the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s).  The card's name and power limit are read in the same
-run.  Prints one JSON line."""
+Per stage of the C++ step driver: milliseconds per call from its CUDA events over the timed steps
+(Simulation.enable_stage_timing); per fluid stage also the algorithmic bytes per node the stage must move (computed
+here from the array shapes, fp64), the achieved rate and its fraction of the H100 SXM data-sheet HBM3 bandwidth
+(3.35 TB/s).  The card's name and power limit are read in the same run.  Prints one JSON line."""
 import argparse
 import json
 import os
@@ -45,7 +45,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_fluid: needs a CUDA device")
     wl = workloads.langmuir_fluid_3d(n=a.n)
-    sim = Simulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=1, native_driver=False)
+    sim = Simulation(wl["n_cell"], wl["prob_lo"], wl["prob_hi"], nox=1)
     for f in wl["fluids"]:
         sim.add_fluid_species(f["name"], f["q"], f["m"], f["density"], f["momentum"])
     sim.Evolve(a.warmup, synchronize_last=False)

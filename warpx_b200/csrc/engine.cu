@@ -22,8 +22,8 @@
 // Multi-rank (one process per GPU, one brick per rank, pic_engine_set_comm): the guard-cell
 // exchanges and the particle migration go through NCCL send/recv on the same stream (csrc/comm.cu),
 // as three axis sweeps with two neighbours each; the host reads 32 bytes once per step (new particle
-// count, overflow status, peak migration count).  warpx_b200/engine.py keeps a Python mirror of the
-// same sequence (torch.distributed transport) for per-stage timing and as a cross-check.
+// count, overflow status, peak migration count).  warpx_b200/engine.py::Simulation drives every run
+// through this driver; per-stage timing is pic_engine_enable_timing / pic_engine_stage_ms.
 #include "pic_common.cuh"
 #include "comm.cuh"
 #include <cmath>
@@ -73,10 +73,11 @@ struct Laser {
 // Per-stage CUDA-event timing of the step driver (pic_engine_enable_timing / pic_engine_stage_ms): the events are
 // recorded on the stream the stages are launched on, inside the same pic_engine_evolve calls a benchmark times.
 enum { ST_FILL_EB = 0, ST_GATHER_PUSH, ST_ZERO_J, ST_DEPOSIT, ST_SYNC_J, ST_EVOLVE_B, ST_FILL_B, ST_EVOLVE_E, ST_FILL_E,
-       ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_FLUID, ST_COUNT };
+       ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_FLUID_GATHER_PUSH, ST_FLUID_FILL,
+       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COUNT };
 static const char* const stage_names[ST_COUNT] = {"fill_boundary_eb", "gather_push", "zero_j", "deposit", "sync_current",
     "evolve_b", "fill_boundary_b", "evolve_e", "fill_boundary_e", "wrap", "migrate", "sort", "nci_filter", "move_window", "push_p", "filter_j",
-    "fluid"};
+    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit"};
 // Cold fluid species (WarpXFluidContainer): two borrowed states of N, NUx, NUy, NUz; the advection writes one from the
 // other and `cur` names the current one.
 struct Fluid {
@@ -667,10 +668,11 @@ static int apply_particle_boundaries(Engine& e, void* stream) {
 // other state, DepositCurrent into the J the particles deposit into (filtered afterwards like theirs).
 static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
     pic_fab* U = fl.U[fl.cur];
-    ENG_CALL(pic_fluid_gather_push(U, &e.fab[0], &e.fab[3], fl.q, fl.m, e.dt, s));
-    for (int d = 0; d < 3; ++d) ENG_CALL(halo_sweep(e, U, 4, d, 2, 0, s));
-    ENG_CALL(pic_fluid_advect(U, fl.U[1 - fl.cur], e.dx, e.dt, nullptr, s));
+    { Stage t(e, ST_FLUID_GATHER_PUSH, s); ENG_CALL(pic_fluid_gather_push(U, &e.fab[0], &e.fab[3], fl.q, fl.m, e.dt, s)); }
+    { Stage t(e, ST_FLUID_FILL, s); for (int d = 0; d < 3; ++d) ENG_CALL(halo_sweep(e, U, 4, d, 2, 0, s)); }
+    { Stage t(e, ST_FLUID_ADVECT, s); ENG_CALL(pic_fluid_advect(U, fl.U[1 - fl.cur], e.dx, e.dt, nullptr, s)); }
     fl.cur = 1 - fl.cur;
+    Stage t(e, ST_FLUID_DEPOSIT, s);
     return pic_fluid_deposit_current(fl.U[fl.cur], e.use_filter ? e.jdep : &e.fab[6], fl.q, s);
 }
 
@@ -686,7 +688,7 @@ static int one_step(Engine& e, bool last, void* s) {
     }
     // ---- OneStep_nosub ----
     ENG_CALL(push_particles_and_deposit(e, s));
-    for (auto& fl : e.fluids) { Stage t(e, ST_FLUID, s); ENG_CALL(evolve_fluid(e, fl, s)); }   // myfl->Evolve, :1171-1178
+    for (auto& fl : e.fluids) ENG_CALL(evolve_fluid(e, fl, s));      // myfl->Evolve, :1171-1178
     if (e.use_filter) { Stage t(e, ST_FILTER, s); ENG_CALL(pic_apply_filter_multi(e.jdep, &e.fab[6], 3, e.npass, s)); }
     { Stage t(e, ST_SYNC_J, s); ENG_CALL(sync_current(e, s)); }
     { Stage t(e, ST_EVOLVE_B, s); ENG_CALL(evolve_b(e, 0.5 * e.dt, s)); }

@@ -1,26 +1,13 @@
-"""Host-side mirror of the reference's explicit EM-PIC step (single level, periodic, FDTD).
+"""Host side of the reference's explicit EM-PIC step (single level, FDTD): the Simulation object.
 
-Method names, argument meaning and sequencing follow WarpX so that the parity tests read like the
-reference (paths relative to Source/ of ECP-WarpX/WarpX):
-
-    Simulation.Evolve                     <- WarpX::Evolve                     Evolve/WarpXEvolve.cpp:93-347
-    Simulation.ExplicitFillBoundaryEBUpdateAux                                 :473-531
-    Simulation.OneStep_nosub              <- WarpX::OneStep_nosub              :353-455
-    Simulation.PushParticlesandDeposit    <- MultiParticleContainer::Evolve    Particles/MultiParticleContainer.cpp:460-482
-                                             PhysicalParticleContainer::Evolve Particles/PhysicalParticleContainer.cpp:1812-2095
-    Simulation.SyncCurrent                <- WarpX::SyncCurrent/SumBoundaryJ   Parallelization/WarpXComm.cpp:1073-1240,1386-1424
-    Simulation.EvolveB / EvolveE          <- WarpX::EvolveB/E                  FieldSolver/WarpXPushFieldsEM.cpp:877-1011
-    Simulation.FillBoundaryE / B          <- WarpX::FillBoundaryE/B            Parallelization/WarpXComm.cpp:699-827
-    Simulation.Synchronize                <- WarpX::Synchronize                Evolve/WarpXEvolve.cpp:64-91
-    Simulation.HandleParticlesAtBoundaries                                     :533-581
-
-Every stage is one call through the C ABI (include/pic_b200.h) into hand-written sm_90a kernels;
-PyTorch only owns device memory, the stream and (multi-GPU) the NCCL transport.
+The step itself -- WarpX::Evolve, OneStep_nosub, SyncCurrent, Synchronize, HandleParticlesAtBoundaries -- runs in
+the library's C++ step driver; the header of csrc/engine.cu maps each of its functions to the reference's.  Every
+stage is a call through the C ABI (include/pic_b200.h) into hand-written sm_90a kernels.  PyTorch only owns device
+memory and the stream; with several ranks torch.distributed broadcasts the id of the driver's NCCL communicator.
 There is no CPU path: constructing a Simulation without a CUDA device raises.
 """
 import ctypes as C
 import math
-import os
 import weakref
 
 import numpy as np
@@ -153,45 +140,6 @@ def release_comm(dist):
         dist._pic_comm = None
 
 
-class _DeviceOps:
-    """pack/unpack/local guard-cell kernels for parallel.HaloExchanger."""
-
-    def __init__(self, sim):
-        self.sim = weakref.proxy(sim)        # no reference cycle: a dropped Simulation is destroyed at once
-
-    def empty(self, n):
-        return self.sim.torch.empty(n, dtype=self.sim.torch.float64, device=self.sim.device)
-
-    def fill_local(self, fab, dim, ng):
-        s = self.sim
-        check(s.L.pic_fill_boundary_local(C.byref(fab), dim, ng, C.byref(s.geom), s.stream))
-
-    def sum_local(self, fab, dim, ng):
-        s = self.sim
-        check(s.L.pic_sum_boundary_local(C.byref(fab), dim, ng, C.byref(s.geom), s.stream))
-
-    def slab_count(self, fab, dim, ng, mode):
-        return self.sim.L.pic_halo_slab_count(C.byref(fab), dim, ng, mode)
-
-    def pack(self, fab, dim, side, ng, mode, buf):
-        s = self.sim
-        check(s.L.pic_halo_pack(C.byref(fab), dim, side, ng, mode, buf.data_ptr(), s.stream))
-
-    def unpack(self, fab, dim, side, ng, mode, buf):
-        s = self.sim
-        check(s.L.pic_halo_unpack(C.byref(fab), dim, side, ng, mode, buf.data_ptr(), s.stream))
-
-    def pack_multi(self, fabs, dim, ng, mode, buf_lo, buf_hi):
-        s = self.sim
-        arr = (abi.pic_fab * len(fabs))(*fabs)
-        check(s.L.pic_halo_pack_multi(arr, len(fabs), dim, ng, mode, buf_lo.data_ptr(), buf_hi.data_ptr(), s.stream))
-
-    def unpack_multi(self, fabs, dim, ng, mode, buf_lo, buf_hi):
-        s = self.sim
-        arr = (abi.pic_fab * len(fabs))(*fabs)
-        check(s.L.pic_halo_unpack_multi(arr, len(fabs), dim, ng, mode, buf_lo.data_ptr(), buf_hi.data_ptr(), s.stream))
-
-
 class Species:
     NAMES = ("x", "y", "z", "w", "ux", "uy", "uz")
 
@@ -213,18 +161,7 @@ class Species:
             a = arrays[name_]
             src = a if isinstance(a, t.Tensor) else t.from_numpy(np.ascontiguousarray(a, dtype=np.float64))
             self.buf[0][n, :self.np].copy_(src, non_blocking=True)
-        # particles the position push moves out of the (periodic) domain: pic_escape_list
-        ecap = self.capacity // 16 + 65536
-        self.esc_mem = t.zeros(ecap + 1, dtype=t.int32, device=sim.device)
-        self.esc = abi.pic_escape_list()
-        self.esc.count = self.esc_mem.data_ptr()
-        self.esc.idx = self.esc_mem.data_ptr() + 4
-        self.esc.capacity = ecap
-        for d in range(3):
-            self.esc.lo[d] = sim.prob_lo[d] if sim.geom.periodic[d] else -math.inf
-            self.esc.hi[d] = sim.prob_hi[d] if sim.geom.periodic[d] else math.inf
-        self.bins = None          # abi.pic_bins once sorted
-        self.cell_start = None
+        self.cell_start = None    # cell-sort scratch of the C++ driver (Simulation._register_species), none without bins
         self.work = None
 
     def soa(self, which=None):
@@ -272,13 +209,13 @@ class FluidSpecies:
 class Simulation:
     def __init__(self, n_cell, prob_lo, prob_hi, nox, galerkin=1, pusher=abi.PUSHER_BORIS,
                  solver=abi.SOLVER_YEE, cfl=1.0, dt=None, dist=None, sort_interval=4,
-                 tile=(8, 8, 8), use_bins=True, device=None, native_driver=True,
+                 tile=(8, 8, 8), use_bins=True, device=None,
                  use_filter=False, filter_npass=(1, 1, 1), boundaries=None, moving_window=None, nb=None,
                  gamma_boost=1.0, nci_stencils=None):
         """boundaries: abi.pic_boundaries (boundary.field_lo/hi, boundary.particle_lo/hi; default all
         periodic); moving_window: (direction, v/c) == warpx.do_moving_window / moving_window_dir /
         moving_window_v; nb: brick grid (default parallel.brick_grid(world); a moving window needs slabs
-        along its direction, e.g. (1, 1, world)).  Non-periodic runs use the C++ driver."""
+        along its direction, e.g. (1, 1, world)); use_bins=False: no cell sort, the order-agnostic kernels."""
         global _error_source
         self.torch, self.L, self.device = self._backend(device)
         _error_source = self.L
@@ -294,31 +231,22 @@ class Simulation:
         self.dinv = [1.0 / v for v in self.dx]                                   # WarpX::InvCellSize
         self.nox, self.galerkin, self.pusher, self.solver = nox, galerkin, pusher, solver
         self.dt = dt if dt else cfl * max_dt(solver, self.dx)
-        self.st = stencil_coefficients(solver, self.dx)
         self.use_filter, self.filter_npass = bool(use_filter), tuple(int(v) for v in filter_npass)
         self.boundaries, self.moving_window = boundaries, moving_window
         # warpx.gamma_boost with boost_direction = z; prob_lo / prob_hi are boosted-frame values already
         # (ConvertLabParamsToBoost, Source/Utils/WarpXUtil.cpp:180-262)
         self.gamma_boost, self.beta_boost = float(gamma_boost), abi.beta_of_gamma(gamma_boost)
-        if self.gamma_boost > 1.0 and not (native_driver and use_bins):
-            raise NotImplementedError("boosted-frame runs need the C++ driver")
         if boundaries is not None:
             for d in range(3):
                 self.geom.periodic[d] = 1 if boundaries.field_lo[d] == abi.FIELD_PERIODIC else 0
         self.nonperiodic = not all(self.geom.periodic[d] for d in range(3))
-        if (self.nonperiodic or moving_window is not None) and not (native_driver and use_bins):
-            raise NotImplementedError("non-periodic / moving-window runs need the C++ driver")
         # particles.use_fdtd_nci_corr: (stencil_exeybz, stencil_bxbyez) from nci_godfrey_stencils
         self.nci_stencils = nci_stencils
-        if nci_stencils is not None and not (native_driver and use_bins):
-            raise NotImplementedError("the NCI corrector needs the C++ driver")
         self.lasers = []
         self.time = 0.0
         g = guard_cells(nox, self.dt, self.dx, self.use_filter, self.filter_npass, moving_window is not None,
                         nci_stencils is not None)
         self.ng_EB, self.ng_J, self.ng_FG, self.ng_FS = g["ng_EB"], g["ng_J"], g["ng_FG"], g["ng_FS"]
-        self.ng_depos_J = g["ng_depos_J"]
-        self._filter_tmp = None
         self.dec = parallel.Decomposition(self.n_cell, tuple(nb) if nb is not None else parallel.brick_grid(self.world),
                                           self.rank)
         self.box_lo, self.box_hi = self.dec.box_lo, self.dec.box_hi
@@ -333,45 +261,36 @@ class Simulation:
             self.data.append(a)
             descs.append(d)
         self.fab = descs
-        self.E = (abi.pic_fab * 3)(*descs[0:3])
-        self.B = (abi.pic_fab * 3)(*descs[3:6])
-        self.J = (abi.pic_fab * 3)(*descs[6:9])
-        self.halo = parallel.HaloExchanger(self.dec, _DeviceOps(self), dist)
         self.species = []
         self.fluids = []
         self.is_synchronized = True
         self.istep = 0
         self._scratch = t.zeros(8, dtype=t.float64, device=self.device)
-        self.stage_events = None      # {stage: [(start, end), ...]} when enable_stage_timing() is on
         # The step sequence runs in the library's C++ driver (csrc/engine.cu); with several ranks it
         # exchanges guard cells and particles over its own NCCL communicator (csrc/comm.cu; the
-        # 128-byte id is broadcast through torch.distributed, the only thing torch transports then).
-        # This Python mirror of the same sequence is used when per-stage timing is requested
-        # (native_driver=False) and as a cross-check of the C++ driver in the tests.
-        self.native = None
+        # 128-byte id is broadcast through torch.distributed, the only thing torch transports).
         self.comm = None
-        if native_driver and use_bins and (self.world == 1 or os.environ.get("PIC_NATIVE_NCCL", "1") != "0"):
-            self.native = self.L.pic_engine_create(C.byref(self.geom), abi.int3(self.box_lo), abi.int3(self.box_hi),
-                                                   nox, galerkin, pusher, solver, cfl, self.dt, sort_interval,
-                                                   1 if self.use_filter else 0, abi.int3(self.filter_npass))
-            if boundaries is not None:
-                check(self.L.pic_engine_set_boundaries(self.native, C.byref(boundaries)))
-            if moving_window is not None:
-                check(self.L.pic_engine_set_moving_window(self.native, int(moving_window[0]), float(moving_window[1])))
-            if self.gamma_boost > 1.0:
-                check(self.L.pic_engine_set_boost(self.native, self.gamma_boost, self.beta_boost))
-            if nci_stencils is not None:
-                check(self.L.pic_engine_set_nci_corrector(self.native, (C.c_double * 5)(*nci_stencils[0]),
-                                                          (C.c_double * 5)(*nci_stencils[1])))
-            g12 = (C.c_int * 12)()
-            self.L.pic_engine_guards(self.native, g12)
-            assert list(g12) == self.ng_EB + self.ng_J + self.ng_FG + self.ng_FS
-            assert self.L.pic_engine_dt(self.native) == self.dt
-            if self.world > 1:
-                self._sync()
-                self.comm = shared_comm(self.L, dist, t, self.device)
-                check(self.L.pic_engine_set_comm(self.native, self.comm, abi.int3(self.dec.nb)))
-            check(self.L.pic_engine_set_fields(self.native, (abi.pic_fab * 9)(*self.fab)))
+        self.native = self.L.pic_engine_create(C.byref(self.geom), abi.int3(self.box_lo), abi.int3(self.box_hi),
+                                               nox, galerkin, pusher, solver, cfl, self.dt, sort_interval,
+                                               1 if self.use_filter else 0, abi.int3(self.filter_npass))
+        if boundaries is not None:
+            check(self.L.pic_engine_set_boundaries(self.native, C.byref(boundaries)))
+        if moving_window is not None:
+            check(self.L.pic_engine_set_moving_window(self.native, int(moving_window[0]), float(moving_window[1])))
+        if self.gamma_boost > 1.0:
+            check(self.L.pic_engine_set_boost(self.native, self.gamma_boost, self.beta_boost))
+        if nci_stencils is not None:
+            check(self.L.pic_engine_set_nci_corrector(self.native, (C.c_double * 5)(*nci_stencils[0]),
+                                                      (C.c_double * 5)(*nci_stencils[1])))
+        g12 = (C.c_int * 12)()
+        self.L.pic_engine_guards(self.native, g12)
+        assert list(g12) == self.ng_EB + self.ng_J + self.ng_FG + self.ng_FS
+        assert self.L.pic_engine_dt(self.native) == self.dt
+        if self.world > 1:
+            self._sync()
+            self.comm = shared_comm(self.L, dist, t, self.device)
+            check(self.L.pic_engine_set_comm(self.native, self.comm, abi.int3(self.dec.nb)))
+        check(self.L.pic_engine_set_fields(self.native, (abi.pic_fab * 9)(*self.fab)))
 
     def close(self):
         """Destroy the C++ driver of this run (device scratch, events).  The NCCL communicator is the process's shared
@@ -402,34 +321,16 @@ class Simulation:
         self.torch.cuda.synchronize()
 
     def enable_stage_timing(self, on=True):
-        """CUDA events (on the launching stream) around every stage; read with stage_ms().  With the C++ driver the
-        events are recorded inside pic_engine_evolve (pic_engine_enable_timing), otherwise by the Python sequencer."""
-        if self.native:
-            check(self.L.pic_engine_enable_timing(self.native, 1 if on else 0))
-            self._native_timing = bool(on)
-            return
-        self.stage_events = {} if on else None
-
-    def _timed(self, name, fn, *a):
-        if self.stage_events is None:
-            return fn(*a)
-        t = self.torch
-        e0, e1 = t.cuda.Event(enable_timing=True), t.cuda.Event(enable_timing=True)
-        e0.record()
-        r = fn(*a)
-        e1.record()
-        self.stage_events.setdefault(name, []).append((e0, e1))
-        return r
+        """CUDA events (on the launching stream) around every stage, recorded inside pic_engine_evolve
+        (pic_engine_enable_timing; switching on resets the sums); read with stage_ms()."""
+        check(self.L.pic_engine_enable_timing(self.native, 1 if on else 0))
 
     def stage_ms(self):
         """{stage: (average milliseconds per call, calls)} of every timed stage (synchronises)."""
-        if self.native:
-            n = self.L.pic_engine_stage_count()
-            ms, calls = (C.c_double * n)(), (C.c_long * n)()
-            check(self.L.pic_engine_stage_ms(self.native, ms, calls))
-            return {self.L.pic_engine_stage_name(k).decode(): (ms[k] / calls[k], int(calls[k])) for k in range(n) if calls[k]}
-        self._sync()
-        return {k: (sum(a.elapsed_time(b) for a, b in v) / len(v), len(v)) for k, v in self.stage_events.items()}
+        n = self.L.pic_engine_stage_count()
+        ms, calls = (C.c_double * n)(), (C.c_long * n)()
+        check(self.L.pic_engine_stage_ms(self.native, ms, calls))
+        return {self.L.pic_engine_stage_name(k).decode(): (ms[k] / calls[k], int(calls[k])) for k in range(n) if calls[k]}
 
     # ------------------------------------------------------------------------------------
     @property
@@ -446,16 +347,7 @@ class Simulation:
         arrays = dict(x=x, y=y, z=z, w=w, ux=ux, uy=uy, uz=uz)
         cap = int(len(x) * capacity_factor) + (0 if self.world == 1 else 65536)
         sp = Species(self, name, q, m, arrays, cap, ids=ids)
-        self.species.append(sp)
-        if self.native:
-            self._alloc_sort_scratch(sp)
-            a, b = sp.soa(0), sp.soa(1)
-            check(self.L.pic_engine_add_species(self.native, q, m, C.byref(a), C.byref(b), sp.capacity,
-                                                sp.cell_start.data_ptr(), abi.int3(self.tile), sp.work.data_ptr(),
-                                                self.stream))
-            self._sync_from_native()
-        elif self.use_bins:
-            self.SortParticlesByBin(sp)
+        self._register_species(sp)
         return sp
 
     def add_plasma_species(self, name, q, m, injector, capacity):
@@ -463,8 +355,6 @@ class Simulation:
         AddPlasma over the whole domain, PhysicalParticleContainer.cpp:450-454,855-922); with
         injector.do_continuous_injection the moving window keeps refilling the uncovered slab.
         capacity: entries of every particle array (the run must never exceed it)."""
-        if not self.native:
-            raise NotImplementedError("plasma injectors need the C++ driver")
         injector.gamma_boost, injector.beta_boost = self.gamma_boost, self.beta_boost
         empty = np.empty(0)
         sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity))
@@ -486,14 +376,8 @@ class Simulation:
         if n < 0:
             raise RuntimeError("pic_b200: " + self.L.pic_last_error().decode())
         sp.np = int(n)
-        self.species.append(sp)
-        self._alloc_sort_scratch(sp)
-        a, b = sp.soa(0), sp.soa(1)
-        check(self.L.pic_engine_add_species(self.native, q, m, C.byref(a), C.byref(b), sp.capacity,
-                                            sp.cell_start.data_ptr(), abi.int3(self.tile), sp.work.data_ptr(),
-                                            self.stream))
+        self._register_species(sp)
         check(self.L.pic_engine_set_injector(self.native, len(self.species) - 1, C.byref(injector)))
-        self._sync_from_native()
         return sp
 
     def add_beam_species(self, name, q, m, beam, capacity):
@@ -502,8 +386,6 @@ class Simulation:
         450-454,503-677), in the lab frame or mapped into this run's boosted frame at the current time.  Each rank keeps
         the particles of its own brick; ids are creation indices, the same on any decomposition.  A beam is created
         once and never refilled.  capacity: entries of every particle array (the run must never exceed it)."""
-        if not self.native:
-            raise NotImplementedError("beam species need the C++ driver")
         beam.gamma_boost, beam.beta_boost = self.gamma_boost, self.beta_boost
         empty = np.empty(0)
         sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity))
@@ -517,13 +399,7 @@ class Simulation:
         if n < 0:
             raise RuntimeError("pic_b200: " + self.L.pic_last_error().decode())
         sp.np = int(n)
-        self.species.append(sp)
-        self._alloc_sort_scratch(sp)
-        a, b = sp.soa(0), sp.soa(1)
-        check(self.L.pic_engine_add_species(self.native, q, m, C.byref(a), C.byref(b), sp.capacity,
-                                            sp.cell_start.data_ptr(), abi.int3(self.tile), sp.work.data_ptr(),
-                                            self.stream))
-        self._sync_from_native()
+        self._register_species(sp)
         return sp
 
     def add_fluid_species(self, name, q, m, density, momentum):
@@ -531,8 +407,8 @@ class Simulation:
         (Source/Fluids/WarpXFluidContainer.cpp:166-254) in the lab frame over this rank's valid nodes, at
         x = prob_lo + i dx: N = n, NU = n u c.  density(x, y, z) -> n [m^-3] and momentum(x, y, z) -> (ux, uy, uz) in
         units of c are evaluated here on the host in float64, on numpy arrays of node coordinates.  One rank, periodic
-        domains without a moving window or boost, no particle species or antennas (the fluid runs in the C++ driver or
-        in the Python sequencer); other runs are refused before anything is allocated."""
+        domains without a moving window or boost, no particle species or antennas; other runs are refused before
+        anything is allocated."""
         if self.nonperiodic:
             raise NotImplementedError("fluid species: every face must be periodic")
         if self.moving_window is not None:
@@ -552,8 +428,7 @@ class Simulation:
         vals = (n, n * (u[0] * C_LIGHT), n * (u[1] * C_LIGHT), n * (u[2] * C_LIGHT))
         for c in range(4):
             fl.data[0][c][vs].copy_(self.torch.from_numpy(np.array(vals[c], dtype=np.float64)))
-        if self.native:
-            check(self.L.pic_engine_add_fluid_species(self.native, fl.q, fl.m, fl.fabs[0], fl.fabs[1]))
+        check(self.L.pic_engine_add_fluid_species(self.native, fl.q, fl.m, fl.fabs[0], fl.fabs[1]))
         self.fluids.append(fl)
         return fl
 
@@ -566,8 +441,6 @@ class Simulation:
         """lasers.names / <laser>.*: a Gaussian antenna (LaserParticleContainer ctor + InitData,
         LaserParticleContainer.cpp:84-270,369-560).  The antenna particles are generated on the host like
         the reference does and uploaded once."""
-        if not self.native:
-            raise NotImplementedError("laser antennas need the C++ driver")
         t = self.torch
         laser.gamma_boost, laser.beta_boost = self.gamma_boost, self.beta_boost
         dxa, lo, hi = abi.dbl3(self.dx), abi.dbl3(self.prob_lo), abi.dbl3(self.prob_hi)
@@ -598,28 +471,28 @@ class Simulation:
             out = {k: v[order] for k, v in out.items()}
         return out
 
-    def _alloc_sort_scratch(self, sp):
-        t = self.torch
-        nb = self.L.pic_bins_count(abi.int3(self.box_lo), abi.int3(self.box_hi), abi.int3(self.tile))
-        if sp.cell_start is None or sp.cell_start.numel() < nb + 1:
+    def _register_species(self, sp):
+        """Append sp and hand it to the C++ driver.  With use_bins the driver gets the cell-sort scratch and sorts the
+        particles at once; without, it keeps no bins, never sorts and runs the order-agnostic kernels."""
+        self.species.append(sp)
+        cell_start = work = None
+        if self.use_bins:
+            t = self.torch
+            nb = self.L.pic_bins_count(abi.int3(self.box_lo), abi.int3(self.box_hi), abi.int3(self.tile))
             sp.cell_start = t.empty(nb + 1, dtype=t.int32, device=self.device)
-        wb = self.L.pic_sort_workspace_bytes(sp.capacity, nb)
-        if sp.work is None or sp.work.numel() < wb:
-            sp.work = t.empty(wb, dtype=t.uint8, device=self.device)
-        return nb
+            sp.work = t.empty(self.L.pic_sort_workspace_bytes(sp.capacity, nb), dtype=t.uint8, device=self.device)
+            cell_start, work = sp.cell_start.data_ptr(), sp.work.data_ptr()
+        a, b = sp.soa(0), sp.soa(1)
+        check(self.L.pic_engine_add_species(self.native, sp.q, sp.m, C.byref(a), C.byref(b), sp.capacity, cell_start,
+                                            abi.int3(self.tile), work, self.stream))
+        self._sync_from_native()
 
     def _sync_from_native(self):
-        """Mirror the C++ driver's view (current buffer, count, bins) into the Python objects."""
+        """Mirror the C++ driver's view (current buffer, count) into the Python objects."""
         for isp, sp in enumerate(self.species):
             n = C.c_long()
             sp.cur = self.L.pic_engine_species_buffer(self.native, isp, C.byref(n))
             sp.np = n.value
-            bins = abi.pic_bins()
-            for d in range(3):
-                bins.box_lo[d], bins.box_hi[d], bins.tile[d] = self.box_lo[d], self.box_hi[d], self.tile[d]
-            bins.cell_start = sp.cell_start.data_ptr()
-            bins.np_binned = sp.np
-            sp.bins = bins
 
     def lower_corner(self, ng):
         """WarpX::LowerCorner of the box grown by ng (Source/WarpX.cpp:2851-2874; RealBox lo =
@@ -628,227 +501,26 @@ class Simulation:
         xyzmin = [self.prob_lo[d] + self.dx[d] * lo[d] for d in range(3)]
         return abi.dbl3(xyzmin), abi.int3(lo)
 
-    # ---- guard cells -------------------------------------------------------------------
-    def FillBoundaryE(self, ng):
-        self._timed("fill_boundary_e", self.halo.fill_boundary, self.fab[0:3], ng)
-
-    def FillBoundaryB(self, ng):
-        self._timed("fill_boundary_b", self.halo.fill_boundary, self.fab[3:6], ng)
-
-    def FillBoundaryEB(self, ng):
-        """FillBoundaryE + FillBoundaryB with the same ng in one exchange per direction."""
-        self._timed("fill_boundary_eb", self.halo.fill_boundary, self.fab[0:6], ng)
-
-    def SyncCurrent(self):
-        """[ApplyFilterJ ->] SumBoundaryJ (WarpXComm.cpp:1233-1237, 1386-1424): src = ng_depos_J
-        (+ stencil_length-1 with the filter, :1413-1416), all guards of J updated afterwards."""
-        src_ng = list(self.ng_depos_J)
-        if self.use_filter:
-            self._timed("filter", self.ApplyFilterJ)
-            src_ng = [min(a + n, b) for a, n, b in zip(self.ng_depos_J, self.filter_npass, self.ng_J)]
-        self.halo.sum_boundary(self.fab[6:9], src_ng, self.ng_J)
-
-    def ApplyFilterJ(self):
-        """WarpX::ApplyFilterJ (WarpXComm.cpp:1357-1374): filter over the grown box into a temporary,
-        copy back (guards included)."""
-        t = self.torch
-        npass = abi.int3(self.filter_npass)
-        for c in range(6, 9):
-            if self._filter_tmp is None or self._filter_tmp.numel() < self.data[c].numel():
-                self._filter_tmp = t.empty(self.data[c].numel(), dtype=t.float64, device=self.device)
-            tmp = abi.pic_fab.from_buffer_copy(self.fab[c])
-            tmp.p = self._filter_tmp.data_ptr()
-            check(self.L.pic_apply_filter(C.byref(self.fab[c]), C.byref(tmp), npass, self.stream))
-            self.data[c].view(-1).copy_(self._filter_tmp[: self.data[c].numel()])
-
-    # ---- field solver ------------------------------------------------------------------
-    def EvolveB(self, dt):
-        self._timed("evolve_b", lambda: check(self.L.pic_evolve_b(self.B, self.E, C.byref(self.st), dt, self.stream)))
-
-    def EvolveE(self, dt):
-        self._timed("evolve_e", lambda: check(self.L.pic_evolve_e(self.E, self.B, self.J, C.byref(self.st), dt,
-                                                                   self.stream)))
-
-    # ---- particles ---------------------------------------------------------------------
-    def _bins(self, sp):
-        return C.byref(sp.bins) if (self.use_bins and sp.bins is not None) else None
-
-    def PushPX(self, sp, dt, push_position=1):
-        xyzmin, lo = self.lower_corner(self.ng_EB)          # box.grow(ngEB), PhysicalParticleContainer.cpp:2583
-        soa = sp.soa()
-        if push_position:
-            sp.esc_mem[:1].zero_()
-        check(self.L.pic_gather_push(C.byref(soa), 0, sp.np, self.E, self.B, abi.dbl3(self.dinv), xyzmin, lo,
-                                     sp.q, sp.m, dt, self.nox, self.galerkin, self.pusher, push_position,
-                                     self._bins(sp), C.byref(sp.esc), self.stream))
-
-    def PushP(self, dt):
-        for sp in self.species:
-            self.PushPX(sp, dt, push_position=0)
-
-    def DepositCurrent(self, sp, dt, relative_time):
-        xyzmin, lo = self.lower_corner(self.ng_J)           # tilebox.grow(ng_J), WarpXParticleContainer.cpp:424-479
-        soa = sp.soa()
-        check(self.L.pic_deposit_esirkepov(C.byref(soa), 0, sp.np, self.J, abi.dbl3(self.dinv), xyzmin, lo,
-                                           sp.q, dt, relative_time, self.nox, self._bins(sp), self.stream))
-
-    def PushParticlesandDeposit(self):
-        for c in range(6, 9):
-            self.data[c].zero_()                             # J.setVal(0), MultiParticleContainer.cpp:467-478
-        for sp in self.species:
-            self._timed("gather_push", self.PushPX, sp, self.dt)
-            self._timed("deposit", self.DepositCurrent, sp, self.dt, -0.5 * self.dt)  # relative_time, PhysicalParticleContainer.cpp:2029
-        for fl in self.fluids:                               # myfl->Evolve, WarpXEvolve.cpp:1171-1178
-            self.EvolveFluid(fl)
-
-    def EvolveFluid(self, fl):
-        """WarpXFluidContainer::Evolve (Source/Fluids/WarpXFluidContainer.cpp:257-314) on a periodic domain: GatherAndPush,
-        the FillBoundary of N and NU (ApplyBcFluidsAndComms :413-417), AdvectivePush_Muscl into the other state,
-        DepositCurrent into J."""
-        L, st = self.L, self.stream
-        self._timed("fluid_gather_push", lambda: check(L.pic_fluid_gather_push(fl.state(), self.E, self.B, fl.q, fl.m,
-                                                                                 self.dt, st)))
-        self._timed("fluid_fill_boundary", self.halo.fill_boundary, list(fl.state()), list(FluidSpecies.NG))
-        self._timed("fluid_advect", lambda: check(L.pic_fluid_advect(fl.state(), fl.state(1 - fl.cur), abi.dbl3(self.dx),
-                                                                       self.dt, None, st)))
-        fl.cur = 1 - fl.cur
-        self._timed("fluid_deposit", lambda: check(L.pic_fluid_deposit_current(fl.state(), self.J, fl.q, st)))
-
-    def SortParticlesByBin(self, sp):
-        bins = abi.pic_bins()
-        for d in range(3):
-            bins.box_lo[d], bins.box_hi[d], bins.tile[d] = self.box_lo[d], self.box_hi[d], self.tile[d]
-        self._alloc_sort_scratch(sp)
-        bins.cell_start = sp.cell_start.data_ptr()
-        src, dst = sp.soa(sp.cur), sp.soa(1 - sp.cur)
-        check(self.L.pic_sort_particles_by_cell(C.byref(src), C.byref(dst), C.byref(self.geom), C.byref(bins),
-                                                sp.work.data_ptr(), self.stream))
-        sp.cur = 1 - sp.cur
-        bins.np_binned = sp.np
-        sp.bins = bins
-
-    def _migrate(self, sp):
-        """Neighbour migration after the periodic wrap (AMReX RedistributeLocal(1)), axis sweeps,
-        entirely on the device (csrc/migrate.cu): classify -> pack into fixed-size messages ->
-        NCCL send/recv -> arrivals fill the holes.  One 8-byte host read per sweep (new count)."""
-        t = self.torch
-        cap_max = max(1 << 16, sp.capacity // 256)
-        if getattr(sp, "_mig", None) is None:
-            n = self.L.pic_migrate_message_doubles(cap_max)
-            f64 = dict(dtype=t.float64, device=self.device)
-            sp._mig = dict(cap_max=cap_max, cap=cap_max, counts=t.zeros(2, dtype=t.int32, device=self.device),
-                           idx_lo=t.empty(cap_max, dtype=t.int32, device=self.device),
-                           idx_hi=t.empty(cap_max, dtype=t.int32, device=self.device),
-                           s_lo=t.zeros(n, **f64), s_hi=t.zeros(n, **f64), r_lo=t.zeros(n, **f64), r_hi=t.zeros(n, **f64),
-                           work=t.zeros(self.L.pic_migrate_workspace_bytes(cap_max) // 4, dtype=t.int32, device=self.device),
-                           head=t.zeros(8, dtype=t.int32).pin_memory())
-        m = sp._mig
-        # Messages have a fixed size (count in the header) so that no host round trip is needed
-        # before the NCCL calls.  The size adapts: every rank uses the same capacity, derived from
-        # the largest per-face count ANY rank saw in the previous step (all-reduced below), with 8x
-        # headroom; the first step uses the worst case (one full layer of cells).
-        cap = m["cap"]
-        nmsg = self.L.pic_migrate_message_doubles(cap)
-        # the particle count lives on the device (work[0]) while the sweeps chain; work[1] = sticky
-        # status; work[6] = largest per-face count of this step
-        m["head"].zero_()
-        m["head"][0] = sp.np
-        m["work"][:8].copy_(m["head"], non_blocking=True)
-        np_dev = m["work"][0:1].data_ptr()
-        peak = m["work"][6:7]
-        soa = sp.soa()
-        soa.np = sp.capacity                      # launch bound only: the kernels read the count from np_dev
-        for dim in range(3):
-            if self.dec.spans(dim):
-                continue
-            check(self.L.pic_particles_classify(C.byref(soa), C.byref(self.geom), dim, self.box_lo[dim],
-                                                self.box_hi[dim], 1 if self.dec.nb[dim] == 2 else 0,
-                                                m["counts"].data_ptr(), m["idx_lo"].data_ptr(), m["idx_hi"].data_ptr(),
-                                                cap, np_dev, self.stream))
-            t.maximum(peak, m["counts"].max(), out=peak)
-            check(self.L.pic_migrate_pack(C.byref(soa), m["idx_lo"].data_ptr(), m["counts"][0:1].data_ptr(), cap,
-                                          m["s_lo"].data_ptr(), self.stream))
-            check(self.L.pic_migrate_pack(C.byref(soa), m["idx_hi"].data_ptr(), m["counts"][1:2].data_ptr(), cap,
-                                          m["s_hi"].data_ptr(), self.stream))
-            parallel.exchange(self.dist, self.dec, dim, m["s_lo"][:nmsg], m["s_hi"][:nmsg], m["r_lo"][:nmsg],
-                              m["r_hi"][:nmsg])
-            check(self.L.pic_migrate_unpack(C.byref(soa), m["counts"].data_ptr(), m["idx_lo"].data_ptr(),
-                                            m["idx_hi"].data_ptr(), m["r_lo"].data_ptr(), m["r_hi"].data_ptr(), cap,
-                                            sp.capacity, m["work"].data_ptr(), np_dev, self.stream))
-        self.dist.all_reduce(peak, op=self.dist.ReduceOp.MAX)
-        head = m["work"][:8].tolist()                                       # the one host read of the step
-        np_new, status, seen = int(head[0]), int(head[1]), int(head[6])
-        if status:
-            raise RuntimeError("particle migration overflow on rank %d (status %d, %d particles through one face, "
-                               "message capacity %d): raise capacity_factor" % (self.rank, status, seen, cap))
-        sp.np = np_new
-        want = 1 << max(14, (8 * seen + 1024).bit_length())                 # power of two >= 8 x seen, >= 16384
-        m["cap"] = min(m["cap_max"], want)
-
-    def HandleParticlesAtBoundaries(self, step):
-        for sp in self.species:
-            soa = sp.soa()
-            # amrex enforcePeriodic; only the particles this step's push moved out of the domain
-            self._timed("wrap", lambda: check(self.L.pic_particles_wrap_listed(C.byref(soa), C.byref(self.geom),
-                                                                                C.byref(sp.esc), self.stream)))
-            if self.world > 1:
-                self._timed("migrate", self._migrate, sp)
-            if self.use_bins and self.sort_interval > 0 and (step + 1) % self.sort_interval == 0:
-                self._timed("sort", self.SortParticlesByBin, sp)
-
-    # ---- the step ----------------------------------------------------------------------
-    def ExplicitFillBoundaryEBUpdateAux(self):
-        if self.is_synchronized:
-            self.FillBoundaryEB(self.ng_EB)                                      # ng_alloc_EB, :487-488
-            self.PushP(-0.5 * self.dt)                                           # :492-504
-            self.is_synchronized = False
-        else:
-            self.FillBoundaryEB(self.ng_FG)                                      # :515-516
-
-    def OneStep_nosub(self):
-        self.PushParticlesandDeposit()
-        self._timed("sync_current", self.SyncCurrent)
-        self.EvolveB(0.5 * self.dt)
-        self.FillBoundaryB(self.ng_FS)
-        self.EvolveE(self.dt)
-        self.FillBoundaryE(self.ng_FS)
-        self.EvolveB(0.5 * self.dt)
-
-    def Synchronize(self):
-        self.FillBoundaryEB(self.ng_FG)
-        self.PushP(0.5 * self.dt)
-        self.is_synchronized = True
-
     def Evolve(self, numsteps, synchronize_last=True):
-        if self.native:
-            check(self.L.pic_engine_evolve(self.native, numsteps, 1 if synchronize_last else 0, self.stream))
-            self.istep += numsteps
-            self.is_synchronized = bool(synchronize_last)
-            self._sync_from_native()
-            for i, fl in enumerate(self.fluids):
-                fl.cur = self.L.pic_engine_fluid_state(self.native, i)
-            # the moving window translates the problem domain; t_new
-            dom = (C.c_double * 6)()
-            self.L.pic_engine_prob_domain(self.native, dom)
-            self.prob_lo, self.prob_hi = tuple(dom[0:3]), tuple(dom[3:6])
-            for d in range(3):
-                self.geom.prob_lo[d], self.geom.prob_hi[d] = dom[d], dom[3 + d]
-            self.time = self.L.pic_engine_time(self.native)
-            return
-        for n in range(numsteps):
-            self.ExplicitFillBoundaryEBUpdateAux()
-            self.OneStep_nosub()
-            if synchronize_last and n == numsteps - 1:
-                self.Synchronize()
-            step = self.istep
-            self.istep += 1
-            self.HandleParticlesAtBoundaries(step)
+        """WarpX::Evolve: numsteps steps of the C++ driver (pic_engine_evolve), then its view mirrored here."""
+        check(self.L.pic_engine_evolve(self.native, numsteps, 1 if synchronize_last else 0, self.stream))
+        self.istep += numsteps
+        self.is_synchronized = bool(synchronize_last)
+        self._sync_from_native()
+        for i, fl in enumerate(self.fluids):
+            fl.cur = self.L.pic_engine_fluid_state(self.native, i)
+        # the moving window translates the problem domain; t_new
+        dom = (C.c_double * 6)()
+        self.L.pic_engine_prob_domain(self.native, dom)
+        self.prob_lo, self.prob_hi = tuple(dom[0:3]), tuple(dom[3:6])
+        for d in range(3):
+            self.geom.prob_lo[d], self.geom.prob_hi[d] = dom[d], dom[3 + d]
+        self.time = self.L.pic_engine_time(self.native)
 
     def set_step(self, istep, time):
         """Restart: continue counting steps (cell-sort cadence) and time from a checkpoint."""
         self.istep, self.time = int(istep), float(time)
-        if self.native:
-            check(self.L.pic_engine_set_step(self.native, int(istep), float(time)))
+        check(self.L.pic_engine_set_step(self.native, int(istep), float(time)))
 
     # ---- diagnostics -------------------------------------------------------------------
     def field_energy(self):

@@ -1,19 +1,11 @@
-"""Box decomposition and neighbour exchange schedule (one rank per GPU, one box per rank).
+"""Box decomposition: one rank per GPU, one box per rank.
 
-Mirrors what WarpX obtains from AMReX's BoxArray/DistributionMapping + FabArray::FillBoundary /
-SumBoundary + ParticleContainer::Redistribute (reference call sites:
-Source/Parallelization/WarpXComm.cpp:699-827, 1386-1424; Source/Evolve/WarpXEvolve.cpp:550-559),
-re-designed for an NVSwitch node: the domain is cut into a brick grid nb[0] x nb[1] x nb[2]
-(2 GPUs 2x1x1, 4 GPUs 2x2x1, 8 GPUs 2x2x2, SURVEY.md section 8e); every exchange is three axis sweeps
-with at most two neighbours each, implemented as pack kernel -> NCCL send/recv -> unpack(+add)
-kernel.  Axes along which a rank spans the whole (periodic) domain use the local kernels instead.
-
-The schedule is device-agnostic: pack/unpack are callables, the transport is torch.distributed
-(NCCL on GPUs, gloo in the CPU tests).
+The domain is cut into a brick grid nb[0] x nb[1] x nb[2] (2 GPUs 2x1x1, 4 GPUs 2x2x1, 8 GPUs 2x2x2,
+SURVEY.md section 8e), the layout WarpX obtains from AMReX's BoxArray / DistributionMapping.  The
+guard-cell exchanges and the particle migration between the bricks run in the C++ step driver
+(csrc/engine.cu, over NCCL); this module only says which brick a rank owns.
 """
 from dataclasses import dataclass
-
-import numpy as np
 
 
 def brick_grid(world_size):
@@ -55,110 +47,3 @@ class Decomposition:
         c = list(self.coord)
         c[dim] += 1 if side else -1
         return self.rank_of(c)
-
-    def spans(self, dim):
-        return self.nb[dim] == 1
-
-
-def exchange(dist, dec, dim, send_lo, send_hi, recv_lo, recv_hi, tag_base=0):
-    """Send `send_lo` to the low neighbour and `send_hi` to the high neighbour along `dim`;
-    receive into recv_lo (from the low neighbour) and recv_hi (from the high neighbour)."""
-    lo, hi = dec.neighbour(dim, 0), dec.neighbour(dim, 1)
-    ops = []
-    # a message travelling "upwards" (sent to hi, received from lo) carries tag_base, the other +1
-    if send_hi is not None and send_hi.numel():
-        ops.append(dist.P2POp(dist.isend, send_hi, hi, tag=tag_base))
-    if recv_lo is not None and recv_lo.numel():
-        ops.append(dist.P2POp(dist.irecv, recv_lo, lo, tag=tag_base))
-    if send_lo is not None and send_lo.numel():
-        ops.append(dist.P2POp(dist.isend, send_lo, lo, tag=tag_base + 1))
-    if recv_hi is not None and recv_hi.numel():
-        ops.append(dist.P2POp(dist.irecv, recv_hi, hi, tag=tag_base + 1))
-    if ops:
-        for req in dist.batch_isend_irecv(ops):
-            req.wait()
-
-
-class HaloExchanger:
-    """FillBoundary / SumBoundary of one field component as axis sweeps.
-
-    ops must provide
-        fill_local(fab, dim, ng), sum_local(fab, dim, src_ng)
-        slab_count(fab, dim, ng, mode) -> int
-        pack(fab, dim, side, ng, mode, buf), unpack(fab, dim, side, ng, mode, buf)
-        empty(n) -> 1-D float64 tensor on the right device
-    """
-
-    def __init__(self, dec, ops, dist=None):
-        self.dec, self.ops, self.dist = dec, ops, dist
-        self._bufs = {}
-
-    def _buf(self, key, n):
-        b = self._bufs.get(key)
-        if b is None or b.numel() < n:
-            b = self.ops.empty(n)
-            self._bufs[key] = b
-        return b[:n]
-
-    def _sweep(self, fabs, dim, ng, mode):
-        if ng == 0 and mode == 0:
-            return
-        if self.dec.spans(dim):
-            for fab in fabs:
-                if mode == 0:
-                    self.ops.fill_local(fab, dim, ng)
-                else:
-                    self.ops.sum_local(fab, dim, ng)
-            return
-        # one message per direction carries the slabs of ALL components (fewer, larger NCCL calls);
-        # pack -> send/recv -> unpack are ordered by the stream, no host synchronisation
-        counts = [self.ops.slab_count(fab, dim, ng, mode) for fab in fabs]
-        n = sum(counts)
-        s_lo, s_hi = self._buf(("s", 0), n), self._buf(("s", 1), n)
-        r_lo, r_hi = self._buf(("r", 0), n), self._buf(("r", 1), n)
-        fused = hasattr(self.ops, "pack_multi") and len(fabs) <= 8
-        if fused:                      # one launch for all components and both sides
-            self.ops.pack_multi(fabs, dim, ng, mode, s_lo, s_hi)
-        else:
-            o = 0
-            for fab, c in zip(fabs, counts):
-                self.ops.pack(fab, dim, 0, ng, mode, s_lo[o:o + c])
-                self.ops.pack(fab, dim, 1, ng, mode, s_hi[o:o + c])
-                o += c
-        exchange(self.dist, self.dec, dim, s_lo, s_hi, r_lo, r_hi)
-        if fused:
-            self.ops.unpack_multi(fabs, dim, ng, mode, r_lo, r_hi)
-        else:
-            o = 0
-            for fab, c in zip(fabs, counts):
-                self.ops.unpack(fab, dim, 0, ng, mode, r_lo[o:o + c])
-                self.ops.unpack(fab, dim, 1, ng, mode, r_hi[o:o + c])
-                o += c
-
-    def fill_boundary(self, fabs, ng):
-        """FillBoundary(ng) of a list of components: guards <- valid points of the periodic image /
-        neighbour.  Axis sweeps x, y, z; every slab spans the full extent of the other axes."""
-        fabs = fabs if isinstance(fabs, (list, tuple)) else [fabs]
-        for dim in range(3):
-            self._sweep(fabs, dim, int(ng[dim]), 0)
-
-    def sum_boundary(self, fabs, src_ng, dst_ng):
-        """SumBoundary(src_ng, dst_ng): fold guards (and shared nodes) into valid points, then
-        refresh dst_ng guards with the sums (WarpXSumGuardCells.cpp:22-23 updates all guards)."""
-        fabs = fabs if isinstance(fabs, (list, tuple)) else [fabs]
-        for dim in range(3):
-            self._sweep(fabs, dim, int(src_ng[dim]), 1)
-        if max(dst_ng) > 0:
-            self.fill_boundary(fabs, dst_ng)
-
-
-def particle_destinations(cell, dec, dim):
-    """(down, up) masks: whether a particle whose (wrapped) cell index along `dim` is `cell` goes
-    to the low / high neighbour (particles move < 1 cell per step, so after the periodic wrap they
-    are at most one brick away; WarpXEvolve.cpp:550-559 RedistributeLocal(1)).  With two bricks
-    both neighbours are the same rank: everything leaving travels on the `up` channel."""
-    owner = cell // dec.width[dim]
-    me, nb = dec.coord[dim], dec.nb[dim]
-    up = (owner == (me + 1) % nb) & (owner != me)
-    down = (owner == (me - 1) % nb) & (owner != me) & ~up
-    return down, up
