@@ -183,13 +183,28 @@ def host_simulation_class():
 FAKE_NCCL = os.path.join(HERE, "_build", "libpic_fake_nccl.so")
 
 
-def build_fake_nccl():
+def _build_nccl_standin(out, defines):
     src = os.path.join(HERE, "fake_nccl.cpp")
-    if not os.path.exists(FAKE_NCCL) or os.path.getmtime(src) > os.path.getmtime(FAKE_NCCL):
-        os.makedirs(os.path.dirname(FAKE_NCCL), exist_ok=True)
-        subprocess.run(["/usr/bin/g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread", "-o", FAKE_NCCL, src],
-                       check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
-    return FAKE_NCCL
+    if not os.path.exists(out) or os.path.getmtime(src) > os.path.getmtime(out):
+        os.makedirs(os.path.dirname(out), exist_ok=True)
+        tmp = "%s.tmp.%d" % (out, os.getpid())
+        subprocess.run(["/usr/bin/g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-pthread"] + defines +
+                       ["-o", tmp, src, "-ldl"], check=True, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
+        os.replace(tmp, out)
+    return out
+
+
+def build_fake_nccl():
+    return _build_nccl_standin(FAKE_NCCL, [])
+
+
+# The same stand-in over DEVICE buffers (-DPIC_STANDIN_DEVICE): ranks as threads of one process driving the real
+# library on one GPU, each on its own stream (tests/test_gpu_multirank.py).
+DEVICE_NCCL = os.path.join(HERE, "_build", "libpic_standin_nccl_device.so")
+
+
+def build_device_nccl():
+    return _build_nccl_standin(DEVICE_NCCL, ["-DPIC_STANDIN_DEVICE"])
 
 
 class ThreadDist:

@@ -517,3 +517,21 @@ def test_eight_bricks_keep_gauss_law(orc, hh):
     0.3 c: particles cross to face, edge and corner neighbours), 8 steps."""
     full = workloads.uniform_plasma_3d(n=16, ppc=(2, 1, 1), u_th=0.3, perturbation=0.01)
     assert gauss_bricks(orc, hh, full, 8, 3, (1, 4, 5, 8), use_filter=True)
+
+
+def test_nccl_standins_export_the_nccl_entry_points(hh):
+    """Both builds of fake_nccl.cpp -- host buffers (the ranks above) and device buffers (tests/test_gpu_multirank.py,
+    -DPIC_STANDIN_DEVICE) -- export the nine symbols csrc/comm.cu binds, and the call counters a test reads to prove the
+    stand-in was the library bound."""
+    import subprocess
+    want = {"ncclGetUniqueId", "ncclCommInitRank", "ncclCommDestroy", "ncclSend", "ncclRecv", "ncclGroupStart",
+            "ncclGroupEnd", "ncclAllReduce", "ncclGetErrorString"}
+    counters = {"standin_sends", "standin_recvs", "standin_allreduces"}
+    for path in (hh.build_fake_nccl(), hh.build_device_nccl()):
+        out = subprocess.run(["nm", "-D", "--defined-only", path], check=True, capture_output=True, text=True).stdout
+        names = {line.split()[-1] for line in out.splitlines() if line.split()[1:2] == ["T"]}
+        assert {n for n in names if n.startswith("nccl")} == want, path
+        assert counters <= names, path
+    # the device build binds the driver API at run time only: no CUDA library at link time
+    out = subprocess.run(["readelf", "-d", hh.build_device_nccl()], check=True, capture_output=True, text=True).stdout
+    assert "libcuda" not in out and "libcudart" not in out

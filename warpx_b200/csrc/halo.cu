@@ -80,7 +80,7 @@ __global__ void slab_kernel(FabView F, double* __restrict__ buf, Slab sl, long t
 }
 
 // all components of an exchange in ONE launch per direction (pack) / per direction (unpack):
-// blockIdx.y = side, the x-grid walks the concatenated slabs of up to PIC_HALO_MAX_FABS components
+// side = side0 + blockIdx.y, the x-grid walks the concatenated slabs of up to PIC_HALO_MAX_FABS components
 constexpr int HALO_MAX = 8;
 struct MultiSlab {
     FabView v[HALO_MAX];
@@ -89,10 +89,10 @@ struct MultiSlab {
     int n;
 };
 __global__ void multi_slab_kernel(MultiSlab m, double* __restrict__ buf_lo, double* __restrict__ buf_hi,
-                                  int dir, int add) {
+                                  int dir, int add, int side0) {
     const long t = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= m.off[m.n]) return;
-    const int side = blockIdx.y;
+    const int side = side0 + blockIdx.y;
     int f = 0;
 #pragma unroll
     for (int q = 1; q < HALO_MAX; ++q) if (q < m.n && t >= m.off[q]) f = q;
@@ -264,9 +264,14 @@ extern "C" long pic_halo_slab_count(const pic_fab* f, int dim, int ng, int mode)
     return n * (mode == 0 ? ng : (mode == 1 ? ng + f->stag[dim] : 2 * ng + f->stag[dim]));
 }
 
+// cells of the box along dim
+static int box_cells(const pic_fab& f, int dim) { return vhi(f, dim) - vlo(f, dim) + 1 - f.stag[dim]; }
+
 static int slab_launch(const pic_fab* f, int dim, int side, int ng, int mode, double* buf, int unpack, void* stream) {
     PIC_REQUIRE(dim >= 0 && dim < 3 && (side == 0 || side == 1) && (mode == 0 || mode == 1), "pic_halo: bad arguments");
-    PIC_REQUIRE(ng <= f->ng[dim], "pic_halo: ng=%d exceeds allocated guards", ng);
+    PIC_REQUIRE(ng >= 0 && ng <= f->ng[dim], "pic_halo: ng=%d exceeds allocated guards", ng);
+    // a wider slab would reach through the valid points into the guards of the other face
+    PIC_REQUIRE(ng <= box_cells(*f, dim), "pic_halo: ng=%d exceeds the %d cells of the box", ng, box_cells(*f, dim));
     Slab sl; full_extent(*f, sl); sl.dim = dim;
     int first, count;
     slab_range(*f, dim, side, ng, mode, unpack, first, count);
@@ -286,28 +291,41 @@ static int multi_launch(const pic_fab* fabs, int nfab, int dim, int ng, int mode
     MultiSlab m;
     m.n = nfab;
     m.off[0] = 0;
+    bool overlap = false;      // the two sides' slabs share points of some component
     for (int f = 0; f < nfab; ++f) {
-        PIC_REQUIRE(ng <= fabs[f].ng[dim], "pic_halo_*_multi: ng=%d exceeds allocated guards", ng);
-        PIC_REQUIRE(mode != 2 || 2 * ng + fabs[f].stag[dim] <= vhi(fabs[f], dim) - vlo(fabs[f], dim) + 1 - fabs[f].stag[dim],
+        const int cells = box_cells(fabs[f], dim);
+        PIC_REQUIRE(ng >= 0 && ng <= fabs[f].ng[dim], "pic_halo_*_multi: ng=%d exceeds allocated guards", ng);
+        PIC_REQUIRE(mode == 2 || ng <= cells, "pic_halo_*_multi: ng=%d exceeds the %d cells of the box", ng, cells);
+        PIC_REQUIRE(mode != 2 || 2 * ng + fabs[f].stag[dim] <= cells,
                     "pic_halo_*_multi: the box is too thin for the fused sum + refresh (ng=%d)", ng);
         m.v[f] = make_view(fabs[f]);
         long cnt = 0;
+        int first[2], count[2];
         for (int side = 0; side < 2; ++side) {
             Slab& sl = m.sl[side][f];
             full_extent(fabs[f], sl); sl.dim = dim;
-            int first, count;
-            slab_range(fabs[f], dim, side, ng, mode, unpack, first, count);
-            sl.start[dim] = first; sl.n[dim] = count;
+            slab_range(fabs[f], dim, side, ng, mode, unpack, first[side], count[side]);
+            sl.start[dim] = first[side]; sl.n[dim] = count[side];
             cnt = (long)sl.n[0] * sl.n[1] * sl.n[2];
         }
+        if (count[0] > 0 && count[1] > 0 && first[0] + count[0] > first[1]) overlap = true;
         m.off[f + 1] = m.off[f] + cnt;
     }
     for (int f = nfab; f < HALO_MAX; ++f) m.off[f + 1] = m.off[nfab];
     const long total = m.off[nfab];
     if (total == 0) return 0;
-    dim3 grid((unsigned)((total + 255) / 256), 2, 1);
-    multi_slab_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(m, buf_lo, buf_hi, unpack, mode);
-    count_launch();
+    const unsigned gx = (unsigned)((total + 255) / 256);
+    if (unpack && overlap) {
+        // Thin boxes (SumBoundary with cells <= 2 ng + stag - 1): a point in both slabs gets the adds of both sides.
+        // One launch per side, low then high, so that no two threads of a launch update the same point and the
+        // order of the two adds is fixed.
+        for (int side = 0; side < 2; ++side)
+            multi_slab_kernel<<<dim3(gx, 1, 1), 256, 0, (cudaStream_t)stream>>>(m, buf_lo, buf_hi, unpack, mode, side);
+        count_launch(2);
+    } else {
+        multi_slab_kernel<<<dim3(gx, 2, 1), 256, 0, (cudaStream_t)stream>>>(m, buf_lo, buf_hi, unpack, mode, 0);
+        count_launch();
+    }
     return check_launch("pic_halo_pack/unpack_multi") ? 0 : 1;
 }
 
