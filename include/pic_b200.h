@@ -222,6 +222,18 @@ int pic_gather_push(const pic_soa* p, long offset, long np,
                     int nox, int galerkin, int pusher, int push_position,
                     const pic_bins* bins, const pic_escape_list* escaped, void* stream);
 
+/* PushPX that also carries out a pending cell sort: particle `pos` of the binned order is read from
+ * in[src[pos]] (src, cell_start of `bins` from pic_sort_index_by_cell on `in`; bins->np_binned = in->np),
+ * pushed, and written to out[pos] together with its weight and id; `in` is left as it was.  `escaped` lists
+ * indices of `out`.  Same arithmetic per particle as pic_sort_apply_permutation followed by pic_gather_push on
+ * `out`.  Served by the default supercell kernel only: orders 1..3 and PIC_GATHER_TILE, anything else is an error
+ * (apply the permutation, then call pic_gather_push). */
+int pic_gather_push_permuted(const pic_soa* in, const pic_soa* out, const int* src,
+                             const pic_fab E[3], const pic_fab B[3],
+                             const double dinv[3], const double xyzmin[3], const int lo[3],
+                             double q, double m, double dt, int nox, int galerkin, int pusher,
+                             const pic_bins* bins, const pic_escape_list* escaped, void* stream);
+
 /* Which kernel the cell-sorted (bins != NULL) gather uses.  PIC_GATHER_TILE (default): one particle per lane.
  * PIC_GATHER_PAIRS: a lane takes two particles of one cell and feeds both from one set of shared-memory loads
  * (half the loads per particle); applies where the stencils of all particles of a cell coincide -- order 3 or 1
@@ -402,6 +414,12 @@ long pic_sort_workspace_bytes(long np, long nbins);
 int pic_sort_particles_by_cell(const pic_soa* in, const pic_soa* out, const pic_geom* g,
                                const pic_bins* bins /* cell_start is written */,
                                void* work, void* stream);
+/* The same sort in two halves.  pic_sort_index_by_cell moves nothing: it writes cell_start and the permutation
+ * (*src points into `work`: particle src[pos] of `in` belongs at position pos).  pic_sort_apply_permutation writes
+ * out[pos] = in[src[pos]] for the seven arrays and the id; pic_gather_push_permuted does that move inside the push. */
+int pic_sort_index_by_cell(const pic_soa* in, const pic_geom* g, const pic_bins* bins /* cell_start is written */,
+                           void* work, const int** src, void* stream);
+int pic_sort_apply_permutation(const pic_soa* in, const pic_soa* out, const int* src, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Non-periodic domains: PEC walls, moving window, laser antenna, continuous injection, particle

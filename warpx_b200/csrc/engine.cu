@@ -32,10 +32,16 @@
 
 namespace pic {
 
+extern int g_gather_mode;      // gather_push_tile.cu
+
 struct Species {
     double q, m;
     pic_soa buf[2];        // counting sort permutes buf[cur] -> buf[1-cur]
     int cur;
+    // A sort inside pic_engine_evolve stops at the permutation: bins describe the new order, the particles still lie
+    // in buf[cur] in the old one, and the next gather + push moves them while it reads them anyway.  Everything else
+    // that reads particle arrays calls apply_pending first; no exported call returns with a permutation pending.
+    const int* pending_src = nullptr;
     pic_bins bins;
     bool has_bins;
     void* sort_work;
@@ -364,9 +370,21 @@ static int sync_current(Engine& e, void* s) {
     return 0;
 }
 
+// the move a deferred sort left out: buf[cur] -> buf[1-cur] through the permutation
+static int apply_pending(Species& sp, void* s) {
+    if (!sp.pending_src) return 0;
+    ENG_CALL(pic_sort_apply_permutation(&sp.buf[sp.cur], &sp.buf[1 - sp.cur], sp.pending_src, s));
+    sp.cur = 1 - sp.cur;
+    sp.pending_src = nullptr;
+    return 0;
+}
+
 static int push(Engine& e, Species& sp, double dt, int push_position, void* s) {
     double xyzmin[3]; int lo[3];
     lower_corner(e, e.ng_EB, xyzmin, lo);
+    // only the default supercell kernel of PushPX carries a pending sort; PushP, order 4 and the pair kernels get the
+    // particles moved first
+    if (!(push_position && sp.has_bins && e.nox <= 3 && g_gather_mode == PIC_GATHER_TILE)) ENG_CALL(apply_pending(sp, s));
     const pic_soa& P = sp.buf[sp.cur];
     if (push_position && sp.has_esc) {
         cudaMemsetAsync(sp.esc.count, 0, sizeof(int), (cudaStream_t)s);
@@ -387,6 +405,13 @@ static int push(Engine& e, Species& sp, double dt, int push_position, void* s) {
     }
     // the main push gathers from the NCI-filtered copies (PhysicalParticleContainer.cpp:1900-1911); PushP does not
     const pic_fab* EB = (e.use_nci && push_position) ? e.nci_fab : e.fab;
+    if (sp.pending_src) {
+        const int* src = sp.pending_src;
+        sp.pending_src = nullptr;
+        sp.cur = 1 - sp.cur;
+        return pic_gather_push_permuted(&P, &sp.buf[sp.cur], src, &EB[0], &EB[3], e.dinv, xyzmin, lo, sp.q, sp.m, dt, e.nox,
+                                        e.galerkin, e.pusher, &sp.bins, sp.has_esc ? &sp.esc : nullptr, s);
+    }
     return pic_gather_push(&P, 0, P.np, &EB[0], &EB[3], e.dinv, xyzmin, lo, sp.q, sp.m, dt, e.nox,
                            e.galerkin, e.pusher, push_position, sp.has_bins ? &sp.bins : nullptr,
                            sp.has_esc ? &sp.esc : nullptr, s);
@@ -461,17 +486,17 @@ static int push_particles_and_deposit(Engine& e, void* s) {
     return 0;
 }
 
-static int sort_species(Engine& e, Species& sp, void* s) {
+// defer: leave the move to the next gather + push (sp.pending_src)
+static int sort_species(Engine& e, Species& sp, bool defer, void* s) {
+    ENG_CALL(apply_pending(sp, s));
     pic_soa& in = sp.buf[sp.cur];
-    pic_soa& out = sp.buf[1 - sp.cur];
-    out.np = in.np;
+    sp.buf[1 - sp.cur].np = in.np;
     for (int d = 0; d < 3; ++d) { sp.bins.box_lo[d] = e.box_lo[d]; sp.bins.box_hi[d] = e.box_hi[d]; }
-    ENG_CALL(pic_sort_particles_by_cell(&in, &out, &e.geom, &sp.bins, sp.sort_work, s));
+    ENG_CALL(pic_sort_index_by_cell(&in, &e.geom, &sp.bins, sp.sort_work, &sp.pending_src, s));
     sp.bins.np_binned = in.np;
-    sp.cur = 1 - sp.cur;
     sp.has_bins = true;
     sp.esc_valid = false;
-    return 0;
+    return defer ? 0 : apply_pending(sp, s);
 }
 
 __global__ void peak_kernel(int* peak, const int* counts) { *peak = max(*peak, max(counts[0], counts[1])); }
@@ -676,7 +701,8 @@ static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
     return pic_fluid_deposit_current(fl.U[fl.cur], e.use_filter ? e.jdep : &e.fab[6], fl.q, s);
 }
 
-static int one_step(Engine& e, bool last, void* s) {
+// last: Synchronize() ends the step; defer_sort: another step of the same call follows, its push moves the sorted particles
+static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     // ---- ExplicitFillBoundaryEBUpdateAux ----
     if (e.is_synchronized) {
         { Stage t(e, ST_FILL_EB, s); ENG_CALL(fill_boundary(e, 0, 6, e.ng_EB, s)); }                    // ng_alloc_EB, :487-488
@@ -722,7 +748,7 @@ static int one_step(Engine& e, bool last, void* s) {
     for (auto& sp : e.species) {
         if (e.comm) { Stage t(e, ST_MIGRATE, s); ENG_CALL(migrate(e, sp, s)); }
         const bool due = e.sort_interval > 0 && (step + 1) % e.sort_interval == 0;
-        if (sp.sort_work && (due || (sp.bins_stale && sp.has_bins))) { Stage t(e, ST_SORT, s); ENG_CALL(sort_species(e, sp, s)); }
+        if (sp.sort_work && (due || (sp.bins_stale && sp.has_bins))) { Stage t(e, ST_SORT, s); ENG_CALL(sort_species(e, sp, defer_sort, s)); }
         sp.bins_stale = false;
     }
     if (e.tm.on && e.tm.recs.size() > 4096) collect_timing(e);          // bound the event pool of long runs
@@ -885,7 +911,7 @@ extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa
     if (!e->all_periodic) ENG_CALL(alloc_boundary_scratch(capacity, &sp.bnd_work, &sp.bnd_cap));
     e->species.push_back(sp);
     ENG_CALL(grow_host_counts(*e));
-    if (cell_start && sort_work) return sort_species(*e, e->species.back(), stream);
+    if (cell_start && sort_work) return sort_species(*e, e->species.back(), false, stream);
     return 0;
 }
 // Multi-rank: this rank's brick is box_lo..box_hi of pic_engine_create, rank = coord[0] + nb[0]*(coord[1]
@@ -1087,7 +1113,10 @@ extern "C" int pic_engine_species_buffer(void* h, int isp, long* np) {
 // WarpX::Evolve(numsteps): the last step synchronises u with x when synchronize_last is set
 extern "C" int pic_engine_evolve(void* h, int numsteps, int synchronize_last, void* stream) {
     Engine* e = static_cast<Engine*>(h);
-    for (int n = 0; n < numsteps; ++n) ENG_CALL(one_step(*e, synchronize_last && n == numsteps - 1, stream));
+    for (int n = 0; n < numsteps; ++n) {
+        const bool final_step = n == numsteps - 1;
+        ENG_CALL(one_step(*e, synchronize_last && final_step, !final_step, stream));
+    }
     return 0;
 }
 

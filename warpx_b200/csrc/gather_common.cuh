@@ -25,6 +25,14 @@ struct EscapeView {
         }
     }
 };
+// A pending cell sort for the push to carry out (pic_gather_push_permuted): slot i of the binned order is particle
+// src[i] of `in`.  src == nullptr: no permutation, the push works in place.
+struct PermSrc {
+    SoaView in;
+    const int* __restrict__ src;
+    const uint64_t* __restrict__ id_in;
+    uint64_t* __restrict__ id_out;
+};
 inline EscapeView make_escape(const pic_escape_list* e, int push_position) {
     EscapeView v;
     v.idx = nullptr; v.count = nullptr; v.cap = 0;

@@ -39,6 +39,19 @@ int gather_push_tile_launch(const pic_soa* p, long offset, long np, const pic_fa
                             const pic_fab B[3], const GatherGeom& gg, double qdt2m, double dt,
                             int nox, int galerkin, int pusher, int push_position,
                             const pic_bins* bins, const EscapeView& esc, cudaStream_t s);
+int gather_push_tile_launch(const pic_soa* p, long offset, long np, const pic_fab E[3],
+                            const pic_fab B[3], const GatherGeom& gg, double qdt2m, double dt,
+                            int nox, int galerkin, int pusher, int push_position,
+                            const pic_bins* bins, const EscapeView& esc, const PermSrc& perm, cudaStream_t s);
+
+static GatherGeom make_gather_geom(const pic_fab E[3], const pic_fab B[3], const double dinv[3], const double xyzmin[3],
+                                   const int lo[3]) {
+    GatherGeom gg;
+    for (int d = 0; d < 3; ++d) { gg.dinv[d] = dinv[d]; gg.xyzmin[d] = xyzmin[d]; gg.lo[d] = lo[d]; }
+    for (int c = 0; c < 3; ++c)
+        for (int d = 0; d < 3; ++d) { gg.stag[c][d] = E[c].stag[d]; gg.stag[3 + c][d] = B[c].stag[d]; }
+    return gg;
+}
 }
 
 namespace pic { extern int g_gather_mode; }      // gather_push_tile.cu
@@ -54,10 +67,7 @@ extern "C" int pic_gather_push(const pic_soa* p, long offset, long np, const pic
     PIC_REQUIRE(galerkin == 0 || galerkin == 1, "pic_gather_push: galerkin must be 0/1");
     PIC_REQUIRE(pusher >= 0 && pusher <= 2, "pic_gather_push: unknown particle pusher %d", pusher);
     PIC_REQUIRE(offset >= 0 && offset + np <= p->np, "pic_gather_push: range outside the tile");
-    GatherGeom gg;
-    for (int d = 0; d < 3; ++d) { gg.dinv[d] = dinv[d]; gg.xyzmin[d] = xyzmin[d]; gg.lo[d] = lo[d]; }
-    for (int c = 0; c < 3; ++c)
-        for (int d = 0; d < 3; ++d) { gg.stag[c][d] = E[c].stag[d]; gg.stag[3 + c][d] = B[c].stag[d]; }
+    const GatherGeom gg = make_gather_geom(E, B, dinv, xyzmin, lo);
     const double qdt2m = 0.5 * q * dt / m;
     cudaStream_t s = (cudaStream_t)stream;
     const EscapeView esc = make_escape(escaped, push_position);
@@ -90,4 +100,23 @@ extern "C" int pic_gather_push(const pic_soa* p, long offset, long np, const pic
 #undef PIC_GP
     count_launch();
     return check_launch("pic_gather_push") ? 0 : 1;
+}
+
+extern "C" int pic_gather_push_permuted(const pic_soa* in, const pic_soa* out, const int* src, const pic_fab E[3],
+                                        const pic_fab B[3], const double dinv[3], const double xyzmin[3],
+                                        const int lo[3], double q, double m, double dt, int nox, int galerkin,
+                                        int pusher, const pic_bins* bins, const pic_escape_list* escaped, void* stream) {
+    PIC_REQUIRE(in && out && src && bins, "pic_gather_push_permuted: null argument");
+    PIC_REQUIRE(out->np == in->np && bins->np_binned == in->np, "pic_gather_push_permuted: the permutation covers every particle (in %ld, out %ld, binned %ld)",
+                (long)in->np, (long)out->np, (long)bins->np_binned);
+    PIC_REQUIRE(in->x != out->x, "pic_gather_push_permuted: in and out must be different buffers");
+    PIC_REQUIRE(nox >= 1 && nox <= 3, "pic_gather_push_permuted: the supercell kernel serves orders 1..3, not %d", nox);
+    PIC_REQUIRE(galerkin == 0 || galerkin == 1, "pic_gather_push_permuted: galerkin must be 0/1");
+    PIC_REQUIRE(pusher >= 0 && pusher <= 2, "pic_gather_push_permuted: unknown particle pusher %d", pusher);
+    PIC_REQUIRE(pic::g_gather_mode == PIC_GATHER_TILE, "pic_gather_push_permuted: only the default gather kernel permutes (gather mode %d is set)", pic::g_gather_mode);
+    if (in->np == 0) return 0;
+    PermSrc perm;
+    perm.in = make_soa(*in, 0); perm.src = src; perm.id_in = in->idcpu; perm.id_out = out->idcpu;
+    return gather_push_tile_launch(out, 0, out->np, E, B, make_gather_geom(E, B, dinv, xyzmin, lo), 0.5 * q * dt / m, dt,
+                                   nox, galerkin, pusher, 1, bins, make_escape(escaped, 1), perm, (cudaStream_t)stream);
 }

@@ -9,6 +9,8 @@
 // such lane would drag its whole warp through ~250 dependent global loads -- measured +40% kernel
 // time per step since the last sort): they are appended to a list and a second, order-agnostic
 // kernel pushes them with one thread each.  Any particle order is correct.
+// PERM (pic_gather_push_permuted): the push that follows a cell sort carries out the sort's move.  Slot ip of the
+// binned order is loaded from perm.in at perm.src[ip] and stored, pushed, to P[ip]; nothing else changes.
 //
 // gather_push_pair_kernel (pic_set_gather_mode(PIC_GATHER_PAIRS); order 3 or 1, Galerkin, Yee): the gather
 // is bound by the shared-memory data return (252 LDS.64 per particle = 15.75 clk per particle per SM,
@@ -68,10 +70,10 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 struct StrayList { int* idx; int* count; int cap; };
 
-template <int N, int G, bool YEE, int TX, int TY, int TZ>
+template <int N, int G, bool YEE, int TX, int TY, int TZ, bool PERM = false>
 __global__ void __launch_bounds__(GT_THREADS, 2)
 gather_push_tile_kernel(SoaView P, BinsView bins, GlobalFields gf, GatherGeom gg, double qdt2m,
-                        double dt, int pusher, int push_position, EscapeView esc, StrayList stray) {
+                        double dt, int pusher, int push_position, EscapeView esc, StrayList stray, PermSrc perm) {
     PIC_DYNAMIC_SMEM(double, smem);
     constexpr bool FIXED = TX > 0;
     const int BD0 = FIXED ? TX + 2 * GT_HALO : bins.tile[0] + 2 * GT_HALO;
@@ -114,11 +116,36 @@ gather_push_tile_kernel(SoaView P, BinsView bins, GlobalFields gf, GatherGeom gg
     }
     cp_async_commit();
 
+    // the push touches neither weight nor id: they move here, coalesced, while the field copies are in flight
+    // (four particles per thread and round: the index -> value -> store chains of a round overlap)
+    if constexpr (PERM) {
+        const bool ids = perm.id_in && perm.id_out;
+        for (int i0 = p_begin + threadIdx.x; i0 < p_end; i0 += 4 * GT_THREADS) {
+            int j[4]; double wv[4]; uint64_t iv[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) j[u] = i0 + u * GT_THREADS < p_end ? perm.src[i0 + u * GT_THREADS] : -1;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                wv[u] = j[u] >= 0 ? perm.in.w[j[u]] : 0.0;
+                iv[u] = j[u] >= 0 && ids ? perm.id_in[j[u]] : 0;
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (j[u] >= 0) { P.w[i0 + u * GT_THREADS] = wv[u]; if (ids) perm.id_out[i0 + u * GT_THREADS] = iv[u]; }
+        }
+    }
+    const SoaView& L = PERM ? perm.in : P;                     // where slot i is loaded from, and at which index
+    auto at = [&](int i) -> int { if constexpr (PERM) return perm.src[i]; else return i; };
+    // a particle handed to a list is pushed in place later: with PERM its record has to be in P by then
+    auto hand_on = [&](int i, double xp, double yp, double zp, double ux, double uy, double uz) {
+        if constexpr (PERM) { P.x[i] = xp; P.y[i] = yp; P.z[i] = zp; P.ux[i] = ux; P.uy[i] = uy; P.uz[i] = uz; }
+    };
+
     // software prefetch: the next particle of this thread is requested before the current one is
     // gathered, so the HBM latency overlaps ~700 instructions of shared-memory gather + push
     double nx = 0, ny = 0, nz = 0, nux = 0, nuy = 0, nuz = 0;
     int ip = p_begin + threadIdx.x;
-    if (ip < p_end) { nx = P.x[ip]; ny = P.y[ip]; nz = P.z[ip]; nux = P.ux[ip]; nuy = P.uy[ip]; nuz = P.uz[ip]; }
+    if (ip < p_end) { const int j = at(ip); nx = L.x[j]; ny = L.y[j]; nz = L.z[j]; nux = L.ux[j]; nuy = L.uy[j]; nuz = L.uz[j]; }
     cp_async_wait_all();
     __syncthreads();
 
@@ -155,7 +182,7 @@ gather_push_tile_kernel(SoaView P, BinsView bins, GlobalFields gf, GatherGeom gg
         const bool valid = ip < p_end;
         double xp = nx, yp = ny, zp = nz, ux = nux, uy = nuy, uz = nuz;
         const int in = ip + GT_THREADS;
-        if (in < p_end) { nx = P.x[in]; ny = P.y[in]; nz = P.z[in]; nux = P.ux[in]; nuy = P.uy[in]; nuz = P.uz[in]; }
+        if (in < p_end) { const int j = at(in); nx = L.x[j]; ny = L.y[j]; nz = L.z[j]; nux = L.ux[j]; nuy = L.uy[j]; nuz = L.uz[j]; }
         int row = -1 - lane;
         const bool in_tile = valid && cell_in_tile(xp, yp, zp, row);
         const int row_prev = __shfl_up_sync(0xffffffffu, row, 1), row_next = __shfl_down_sync(0xffffffffu, row, 1);
@@ -163,10 +190,10 @@ gather_push_tile_kernel(SoaView P, BinsView bins, GlobalFields gf, GatherGeom gg
         bool now = valid;
         if (valid && !in_tile) {                  // left the supercell since the sort: second kernel
             const int n = atomicAdd(stray.count, 1);
-            if (n < stray.cap) { stray.idx[n] = ip; now = false; }
+            if (n < stray.cap) { hand_on(ip, xp, yp, zp, ux, uy, uz); stray.idx[n] = ip; now = false; }
         } else if (valid && isolated) {           // changed row inside the supercell: after the sweep
             const int n = atomicAdd(&s_nstray, 1);
-            if (n < GT_LOCAL_STRAYS) { s_stray[n] = ip; now = false; }
+            if (n < GT_LOCAL_STRAYS) { hand_on(ip, xp, yp, zp, ux, uy, uz); s_stray[n] = ip; now = false; }
         }
         __syncwarp();                             // one convergent pass through the 700-instruction body
         if (now) finish(ip, xp, yp, zp, ux, uy, uz, in_tile);
@@ -377,10 +404,11 @@ int g_gather_mode = 0;
 template <int N, int G>
 static int launch(SoaView P, const BinsView& bv, const GlobalFields& gf, const GatherGeom& gg,
                   bool yee, double qdt2m, double dt, int pusher, int push_position, const EscapeView& esc,
-                  cudaStream_t s) {
+                  const PermSrc& perm, cudaStream_t s) {
     const long bvol = (long)(bv.tile[0] + 2 * GT_HALO) * (bv.tile[1] + 2 * GT_HALO) * (bv.tile[2] + 2 * GT_HALO);
     const long tvol = (long)bv.tile[0] * bv.tile[1] * bv.tile[2];
-    const bool pairs = g_gather_mode != 0 && yee && G == 1 && (N == 3 || N == 1);
+    const bool permute = perm.src != nullptr;
+    const bool pairs = !permute && g_gather_mode != 0 && yee && G == 1 && (N == 3 || N == 1);
     const bool wide = g_gather_mode == 2, mid = g_gather_mode == 3;
     const size_t smem = (size_t)6 * bvol * sizeof(double) + (pairs ? sizeof(int) * (size_t)(tvol + 1 + GT_LOCAL_STRAYS + 1) : 0);
     const size_t static_smem = pairs ? 0 : sizeof(int) * (GT_LOCAL_STRAYS + 2);       // s_stray + s_nstray
@@ -390,28 +418,36 @@ static int launch(SoaView P, const BinsView& bv, const GlobalFields& gf, const G
     // stray list (stream-ordered scratch): a few per mille of the particles per step since the sort
     StrayList stray;
     stray.cap = (int)(bv.np_limit / 8 + 1024);
+#define PIC_KARGS P, bv, gf, gg, qdt2m, dt, pusher, push_position, esc, stray
+#define PIC_PERM , perm          /* the supercell kernel's extra argument */
+    // the default kernel: 8x8x8 supercells on the Yee grid are the tuned instance (immediate LDS offsets)
+#define PIC_LAUNCH_TILE \
+    else if (permute && yee && t888) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, PIC_PERM, true, 8, 8, 8, true); \
+    else if (permute && yee) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, PIC_PERM, true, 0, 0, 0, true); \
+    else if (permute) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, PIC_PERM, false, 0, 0, 0, true); \
+    else if (yee && t888) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, PIC_PERM, true, 8, 8, 8); \
+    else if (yee) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, PIC_PERM, true, 0, 0, 0); \
+    else PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, PIC_PERM, false, 0, 0, 0);
 #ifndef PIC_SIMT_HOST
     int* scratch = nullptr;
     if (cudaMallocAsync((void**)&scratch, sizeof(int) * (size_t)(stray.cap + 1), s) != cudaSuccess)
         return fail("pic_gather_push: cannot allocate %ld B of scratch", (long)(sizeof(int) * (stray.cap + 1)));
     stray.count = scratch; stray.idx = scratch + 1;
     cudaMemsetAsync(stray.count, 0, sizeof(int), s);
-#define PIC_LAUNCH_K(KERNEL, THREADS, ...) do { \
+#define PIC_LAUNCH_K(KERNEL, THREADS, EXTRA, ...) do { \
         auto k = KERNEL<N, G, __VA_ARGS__>; \
         if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024 - static_smem - 1024)) != cudaSuccess) \
             return fail("pic_gather_push: cannot raise the dynamic shared memory limit"); \
-        k<<<ntiles, THREADS, smem, s>>>(P, bv, gf, gg, qdt2m, dt, pusher, push_position, esc, stray); } while (0)
+        k<<<ntiles, THREADS, smem, s>>>(PIC_KARGS EXTRA); } while (0)
     if (pairs) {
         if constexpr (G == 1 && (N == 3 || N == 1)) {
-            if (t888 && wide) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, true, 8, 8, 8, 1);
-            else if (t888 && mid) PIC_LAUNCH_K(gather_push_pair_kernel, 192, true, 8, 8, 8, 2, 192);
-            else if (t888) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, true, 8, 8, 8, 2);
-            else PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, true, 0, 0, 0, 2);
+            if (t888 && wide) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, , true, 8, 8, 8, 1);
+            else if (t888 && mid) PIC_LAUNCH_K(gather_push_pair_kernel, 192, , true, 8, 8, 8, 2, 192);
+            else if (t888) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, , true, 8, 8, 8, 2);
+            else PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, , true, 0, 0, 0, 2);
         }
     }
-    else if (yee && t888) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, true, 8, 8, 8);       // the tuned instance: immediate LDS offsets
-    else if (yee) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, true, 0, 0, 0);
-    else PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, false, 0, 0, 0);
+    PIC_LAUNCH_TILE
 #undef PIC_LAUNCH_K
     if (yee) gather_push_listed_kernel<N, G, true><<<NUM_SMS * 8, 128, 0, s>>>(P, stray, gf, gg, qdt2m, dt, pusher, push_position, esc);
     else gather_push_listed_kernel<N, G, false><<<NUM_SMS * 8, 128, 0, s>>>(P, stray, gf, gg, qdt2m, dt, pusher, push_position, esc);
@@ -422,30 +458,31 @@ static int launch(SoaView P, const BinsView& bv, const GlobalFields& gf, const G
     (void)s; (void)t888;
     std::vector<int> scratch((size_t)stray.cap + 1, 0);
     stray.count = scratch.data(); stray.idx = scratch.data() + 1;
-#define PIC_LAUNCH_K(KERNEL, THREADS, ...) \
-        ::simt::launch(dim3(ntiles), dim3(THREADS), smem + 64, [&] { KERNEL<N, G, __VA_ARGS__>(P, bv, gf, gg, qdt2m, dt, pusher, push_position, esc, stray); })
+#define PIC_LAUNCH_K(KERNEL, THREADS, EXTRA, ...) \
+        ::simt::launch(dim3(ntiles), dim3(THREADS), smem + 64, [&] { KERNEL<N, G, __VA_ARGS__>(PIC_KARGS EXTRA); })
     if (pairs) {
         if constexpr (G == 1 && (N == 3 || N == 1)) {
-            if (t888 && wide) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, true, 8, 8, 8, 1);
-            else if (t888 && mid) PIC_LAUNCH_K(gather_push_pair_kernel, 192, true, 8, 8, 8, 2, 192);
-            else if (t888) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, true, 8, 8, 8, 2);
-            else PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, true, 0, 0, 0, 2);
+            if (t888 && wide) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, , true, 8, 8, 8, 1);
+            else if (t888 && mid) PIC_LAUNCH_K(gather_push_pair_kernel, 192, , true, 8, 8, 8, 2, 192);
+            else if (t888) PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, , true, 8, 8, 8, 2);
+            else PIC_LAUNCH_K(gather_push_pair_kernel, GP_THREADS, , true, 0, 0, 0, 2);
         }
     }
-    else if (yee && t888) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, true, 8, 8, 8);
-    else if (yee) PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, true, 0, 0, 0);
-    else PIC_LAUNCH_K(gather_push_tile_kernel, GT_THREADS, false, 0, 0, 0);
+    PIC_LAUNCH_TILE
 #undef PIC_LAUNCH_K
     if (yee) ::simt::launch(dim3(4), dim3(128), 64, [&] { gather_push_listed_kernel<N, G, true>(P, stray, gf, gg, qdt2m, dt, pusher, push_position, esc); });
     else ::simt::launch(dim3(4), dim3(128), 64, [&] { gather_push_listed_kernel<N, G, false>(P, stray, gf, gg, qdt2m, dt, pusher, push_position, esc); });
     return 0;
 #endif
+#undef PIC_LAUNCH_TILE
+#undef PIC_PERM
+#undef PIC_KARGS
 }
 
 int gather_push_tile_launch(const pic_soa* p, long offset, long np, const pic_fab E[3],
                             const pic_fab B[3], const GatherGeom& gg, double qdt2m, double dt,
                             int nox, int galerkin, int pusher, int push_position,
-                            const pic_bins* bins, const EscapeView& esc, cudaStream_t s) {
+                            const pic_bins* bins, const EscapeView& esc, const PermSrc& perm, cudaStream_t s) {
     PIC_REQUIRE(offset == 0 && np == p->np, "pic_gather_push: bins describe the whole tile (offset 0, np = all)");
     BinsView bv = make_bins(*bins);
     bv.np_limit = (int)std::min<long>(bins->np_binned, np);   // the tile may have shrunk since the sort
@@ -453,7 +490,7 @@ int gather_push_tile_launch(const pic_soa* p, long offset, long np, const pic_fa
     for (int c = 0; c < 3; ++c) { gf.v[c] = make_view(E[c]); gf.v[3 + c] = make_view(B[c]); }
     SoaView P = make_soa(*p, 0);
     const bool yee = is_yee(E, B);
-#define PIC_GT(N, G) return launch<N, G>(P, bv, gf, gg, yee, qdt2m, dt, pusher, push_position, esc, s)
+#define PIC_GT(N, G) return launch<N, G>(P, bv, gf, gg, yee, qdt2m, dt, pusher, push_position, esc, perm, s)
     if (nox == 1 && galerkin) PIC_GT(1, 1);
     if (nox == 1) PIC_GT(1, 0);
     if (nox == 2 && galerkin) PIC_GT(2, 1);
@@ -461,6 +498,15 @@ int gather_push_tile_launch(const pic_soa* p, long offset, long np, const pic_fa
     if (nox == 3 && galerkin) PIC_GT(3, 1);
     PIC_GT(3, 0);
 #undef PIC_GT
+}
+
+// the ordinary push: in place, no permutation
+int gather_push_tile_launch(const pic_soa* p, long offset, long np, const pic_fab E[3],
+                            const pic_fab B[3], const GatherGeom& gg, double qdt2m, double dt,
+                            int nox, int galerkin, int pusher, int push_position,
+                            const pic_bins* bins, const EscapeView& esc, cudaStream_t s) {
+    return gather_push_tile_launch(p, offset, np, E, B, gg, qdt2m, dt, nox, galerkin, pusher, push_position, bins, esc,
+                                   PermSrc{}, s);
 }
 
 }  // namespace pic

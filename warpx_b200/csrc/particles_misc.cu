@@ -79,16 +79,23 @@ __global__ void sort_count_kernel(SoaView P, long np, BinsView b, SortGeom sg, i
     warp_aggregated_add(counts, bin, active, &rank);
 }
 
-__global__ void sort_scatter_kernel(SoaView in, SoaView out, const uint64_t* __restrict__ id_in,
-                                    uint64_t* __restrict__ id_out, long np, const int* __restrict__ keys,
-                                    const int* __restrict__ cell_start, int* __restrict__ fill) {
+// the slot of every particle in the binned order, as the permutation src[slot] = particle
+__global__ void sort_index_kernel(long np, const int* __restrict__ keys, const int* __restrict__ cell_start,
+                                  int* __restrict__ fill, int* __restrict__ src) {
     const long ip = (long)blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = ip < np;
     const int bin = active ? keys[ip] : 0;
     int rank;
     const int base = warp_aggregated_add(fill, bin, active, &rank);
-    if (!active) return;
-    const int pos = cell_start[bin] + base + rank;
+    if (active) src[cell_start[bin] + base + rank] = (int)ip;
+}
+
+// out[pos] = in[src[pos]]: coalesced stores; the loads follow src, which is monotone except where particles changed cell
+__global__ void sort_apply_kernel(SoaView in, SoaView out, const uint64_t* __restrict__ id_in,
+                                  uint64_t* __restrict__ id_out, long np, const int* __restrict__ src) {
+    const long pos = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (pos >= np) return;
+    const int ip = src[pos];
     out.x[pos] = in.x[ip]; out.y[pos] = in.y[ip]; out.z[pos] = in.z[ip]; out.w[pos] = in.w[ip];
     out.ux[pos] = in.ux[ip]; out.uy[pos] = in.uy[ip]; out.uz[pos] = in.uz[ip];
     if (id_in && id_out) id_out[pos] = id_in[ip];
@@ -238,19 +245,18 @@ extern "C" long pic_bins_count(const int box_lo[3], const int box_hi[3], const i
 }
 
 extern "C" long pic_sort_workspace_bytes(long np, long nbins) {
-    return (long)(align256((size_t)np * 4) + 2 * align256((size_t)(nbins + 1) * 4) + align256(scan_temp_bytes(nbins + 1)));
+    return (long)(2 * align256((size_t)np * 4) + 2 * align256((size_t)(nbins + 1) * 4) + align256(scan_temp_bytes(nbins + 1)));
 }
 
-extern "C" int pic_sort_particles_by_cell(const pic_soa* in, const pic_soa* out, const pic_geom* g,
-                                          const pic_bins* bins, void* work, void* stream) {
+extern "C" int pic_sort_index_by_cell(const pic_soa* in, const pic_geom* g, const pic_bins* bins, void* work,
+                                      const int** src_out, void* stream) {
     const long np = in->np;
-    PIC_REQUIRE(out->np == np, "pic_sort_particles_by_cell: in/out sizes differ");
-    PIC_REQUIRE(in->x != out->x, "pic_sort_particles_by_cell: in-place sort is not supported");
     BinsView bv = make_bins(*bins);
     const long nbins = bins_count(bv);
-    PIC_REQUIRE(nbins + 1 < (1L << 31) && np < (1L << 31), "pic_sort_particles_by_cell: too many bins/particles for int32");
+    PIC_REQUIRE(nbins + 1 < (1L << 31) && np < (1L << 31), "pic_sort_index_by_cell: too many bins/particles for int32");
     cudaStream_t s = (cudaStream_t)stream;
     char* w = (char*)work;
+    int* src = (int*)w; w += align256((size_t)np * 4);
     int* keys = (int*)w; w += align256((size_t)np * 4);
     int* counts = (int*)w; w += align256((size_t)(nbins + 1) * 4);
     int* fill = (int*)w; w += align256((size_t)(nbins + 1) * 4);
@@ -271,9 +277,29 @@ extern "C" int pic_sort_particles_by_cell(const pic_soa* in, const pic_soa* out,
     cub::DeviceScan::ExclusiveSum(temp, temp_bytes, counts, cell_start, (int)(nbins + 1), s);
     count_launch();
     if (np > 0) {
-        sort_scatter_kernel<<<(unsigned)((np + 255) / 256), 256, 0, s>>>(make_soa(*in, 0), make_soa(*out, 0),
-            in->idcpu, out->idcpu, np, keys, cell_start, fill);
+        sort_index_kernel<<<(unsigned)((np + 255) / 256), 256, 0, s>>>(np, keys, cell_start, fill, src);
         count_launch();
     }
-    return check_launch("pic_sort_particles_by_cell") ? 0 : 1;
+    *src_out = src;
+    return check_launch("pic_sort_index_by_cell") ? 0 : 1;
+}
+
+extern "C" int pic_sort_apply_permutation(const pic_soa* in, const pic_soa* out, const int* src, void* stream) {
+    const long np = in->np;
+    PIC_REQUIRE(out->np == np, "pic_sort_apply_permutation: in/out sizes differ");
+    PIC_REQUIRE(in->x != out->x, "pic_sort_apply_permutation: in-place permutation is not supported");
+    if (np == 0) return 0;
+    sort_apply_kernel<<<(unsigned)((np + 255) / 256), 256, 0, (cudaStream_t)stream>>>(make_soa(*in, 0), make_soa(*out, 0),
+        in->idcpu, out->idcpu, np, src);
+    count_launch();
+    return check_launch("pic_sort_apply_permutation") ? 0 : 1;
+}
+
+extern "C" int pic_sort_particles_by_cell(const pic_soa* in, const pic_soa* out, const pic_geom* g,
+                                          const pic_bins* bins, void* work, void* stream) {
+    PIC_REQUIRE(out->np == in->np, "pic_sort_particles_by_cell: in/out sizes differ");
+    PIC_REQUIRE(in->x != out->x, "pic_sort_particles_by_cell: in-place sort is not supported");
+    const int* src = nullptr;
+    if (int rc = pic_sort_index_by_cell(in, g, bins, work, &src, stream)) return rc;
+    return pic_sort_apply_permutation(in, out, src, stream);
 }

@@ -66,6 +66,8 @@ def bind(L):
         "pic_evolve_e": (C.c_int, [fabp, fabp, fabp, stp, C.c_double, vp]),
         "pic_gather_push": (C.c_int, [soap, C.c_long, C.c_long, fabp, fabp, dp, dp, ip, C.c_double,
                                       C.c_double, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int, bp, escp, vp]),
+        "pic_gather_push_permuted": (C.c_int, [soap, soap, vp, fabp, fabp, dp, dp, ip, C.c_double, C.c_double,
+                                               C.c_double, C.c_int, C.c_int, C.c_int, bp, escp, vp]),
         "pic_particles_wrap_listed": (C.c_int, [soap, gp, escp, vp]),
         "pic_deposit_esirkepov": (C.c_int, [soap, C.c_long, C.c_long, fabp, dp, dp, ip, C.c_double,
                                             C.c_double, C.c_double, C.c_int, bp, vp]),
@@ -92,6 +94,8 @@ def bind(L):
         "pic_bins_count": (C.c_long, [ip, ip, ip]),
         "pic_sort_workspace_bytes": (C.c_long, [C.c_long, C.c_long]),
         "pic_sort_particles_by_cell": (C.c_int, [soap, soap, gp, bp, vp, vp]),
+        "pic_sort_index_by_cell": (C.c_int, [soap, gp, bp, vp, C.POINTER(vp), vp]),
+        "pic_sort_apply_permutation": (C.c_int, [soap, soap, vp, vp]),
         "pic_sum_squares_unique": (C.c_int, [fabp, gp, vp, vp]),
         "pic_particle_energy": (C.c_int, [soap, C.c_double, vp, vp]),
         "pic_engine_create": (vp, [gp, ip, ip, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int,
