@@ -52,8 +52,9 @@ typedef struct pic_soa {
 
 /* Stencil coefficients == FiniteDifferenceSolver::m_stencil_coefs_{x,y,z}
  * (FiniteDifferenceSolver.cpp:30-103).  Yee: c[0] = 1/dx (CartesianYeeAlgorithm.H:37-42).
- * CKC: {1/d, alpha, beta1, beta2, gamma/d} (CartesianCKCAlgorithm.H:84-101). */
-enum { PIC_SOLVER_YEE = 0, PIC_SOLVER_CKC = 1 };
+ * CKC: {1/d, alpha, beta1, beta2, gamma/d} (CartesianCKCAlgorithm.H:84-101).
+ * PIC_SOLVER_NONE: algo.maxwell_solver = none (the step driver only gathers and pushes, WarpXEvolve.cpp:176-182). */
+enum { PIC_SOLVER_YEE = 0, PIC_SOLVER_CKC = 1, PIC_SOLVER_NONE = 2 };
 typedef struct pic_stencil {
     int algo;
     double cx[5]; double cy[5]; double cz[5];
@@ -420,6 +421,9 @@ int pic_sort_particles_by_cell(const pic_soa* in, const pic_soa* out, const pic_
 int pic_sort_index_by_cell(const pic_soa* in, const pic_geom* g, const pic_bins* bins /* cell_start is written */,
                            void* work, const int** src, void* stream);
 int pic_sort_apply_permutation(const pic_soa* in, const pic_soa* out, const int* src, void* stream);
+/* np ints of the sort workspace that only pic_sort_index_by_cell writes: free for other uses until the next sort
+ * (np = the particle count of the last pic_sort_index_by_cell on `work`). */
+int* pic_sort_scratch(void* work, long np);
 
 /* ------------------------------------------------------------------------------------------
  * Non-periodic domains: PEC walls, moving window, laser antenna, continuous injection, particle
@@ -659,6 +663,43 @@ int pic_fluid_deposit_charge(const pic_fab* N, const pic_fab* rho, double q, voi
  * leave the engine unchanged.  pic_engine_fluid_state: which state of fluid i is current (0 = A, 1 = B), -1 if none. */
 int pic_engine_add_fluid_species(void* h, double q, double m, const pic_fab stateA[4], const pic_fab stateB[4]);
 int pic_engine_fluid_state(void* h, int i);
+
+/* ------------------------------------------------------------------------------------------
+ * Binary Coulomb collisions (collisions.collision_names, <name>.type = pairwisecoulomb), 3D Cartesian.
+ * One collision of species 1 with species 2 (the same species when same_species):
+ * PairWiseCoulombCollisionFunc (Source/Particles/Collision/BinaryCollision/Coulomb/PairWiseCoulombCollisionFunc.H)
+ * with its CoulombLog (<= 0: computed per pair) and the run's collision index and random seed.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct pic_coulomb_collision {
+    double q1, m1, q2, m2;
+    double coulomb_log;     /* <name>.CoulombLog; <= 0: computed from the cell's Debye length              */
+    uint64_t seed;          /* key of the Philox4x64-10 streams                                            */
+    int collision_index;    /* position in collisions.collision_names; part of every stream's counter      */
+    int same_species;       /* 1: intra-species (species 2 arguments ignored)                              */
+} pic_coulomb_collision;
+
+/* BinaryCollision::doCollisionsWithinTile (BinaryCollision/BinaryCollision.H:234-750) over the box of the bins, dt =
+ * the collision's dt (dt * ndt, CollisionHandler.cpp:85-93): per cell, density (and temperature,
+ * Coulomb/ComputeTemperature.H), ShuffleFisherYates, the independent pair chains of ElasticCollisionPerez
+ * (Coulomb/ElasticCollisionPerez.H:57-148) and UpdateMomentumPerezElastic (Coulomb/UpdateMomentumPerezElastic.H).
+ * The bins must be current (np_binned == np); src1 / src2: the pending permutation of pic_sort_index_by_cell (slot ->
+ * storage index), NULL when the particles lie in bin order.  Both species' bins describe the same box and tiles.
+ * Only ux, uy, uz change; positions, weights, ids, cell_start and src keep their bits.  The result depends on the
+ * particles of each cell by id, the seed, the collision index, `step` and the global cell, not on storage order
+ * (csrc/collision.cu states the random-stream layout).  scratch1 / scratch2: one device int per particle of each
+ * species (e.g. pic_sort_scratch of its sort workspace), used only by cells of more than 2048 colliding particles;
+ * with NULL such cells are left unchanged and *status (device int, zeroed by the caller) becomes non-zero. */
+int pic_collide_pairwise_coulomb(const pic_coulomb_collision* c, const pic_soa* p1, const pic_bins* b1, const int* src1,
+                                 const pic_soa* p2, const pic_bins* b2, const int* src2, const pic_geom* g, double dt,
+                                 long step, int* scratch1, int* scratch2, int* status, void* stream);
+/* One entry of collisions.collision_names for the step driver (CollisionHandler, Source/Particles/Collision/
+ * CollisionHandler.cpp:26-93): species isp1 with isp2 (the same index: intra-species), <name>.CoulombLog,
+ * <name>.ndt >= 1, the random seed.  Collisions run after ExplicitFillBoundaryEBUpdateAux and before the push
+ * (WarpXEvolve.cpp:141-159), at the steps with int(floor(t / dt)) % ndt == 0, with dt * ndt.  A colliding species is
+ * sorted by cell before its collision whenever its bins are stale.  Species without bins, indices out of range,
+ * ndt < 1, runs with fluid species and runs over several ranks (not yet checked against a single box) are refused
+ * before the engine changes. */
+int pic_engine_add_collision(void* engine, int isp1, int isp2, double coulomb_log, int ndt, uint64_t seed);
 
 /* Number of kernels launched by this library since load (bench.py's gpu_launches). */
 long pic_launch_count(void);

@@ -77,6 +77,12 @@ class pic_gaussian_beam(C.Structure):
                 ("gamma_boost", C.c_double), ("beta_boost", C.c_double)]
 
 
+class pic_coulomb_collision(C.Structure):
+    _fields_ = [("q1", C.c_double), ("m1", C.c_double), ("q2", C.c_double), ("m2", C.c_double),
+                ("coulomb_log", C.c_double), ("seed", C.c_uint64), ("collision_index", C.c_int),
+                ("same_species", C.c_int)]
+
+
 FIELD_PERIODIC, FIELD_PEC = 0, 1
 PARTICLE_PERIODIC, PARTICLE_ABSORBING, PARTICLE_REFLECTING = 0, 1, 2
 _FIELD_BC = {"periodic": FIELD_PERIODIC, "pec": FIELD_PEC}
@@ -175,6 +181,15 @@ def LWFA_SIGNATURES(fabp, soap, gp, bp, lp, jp, dp, ip, vp):
     }
 
 
+def COLLISION_SIGNATURES(soap, bp, gp, vp):
+    """ctypes signatures of the binary-collision entry points of include/pic_b200.h."""
+    return {
+        "pic_collide_pairwise_coulomb": (C.c_int, [C.POINTER(pic_coulomb_collision), soap, bp, vp, soap, bp, vp, gp,
+                                                   C.c_double, C.c_long, vp, vp, vp, vp]),
+        "pic_engine_add_collision": (C.c_int, [vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_uint64]),
+    }
+
+
 def FLUID_SIGNATURES(fabp, dp, vp):
     """ctypes signatures of the fluid-species entry points of include/pic_b200.h (a fluid state is 4 pic_fab)."""
     return {
@@ -187,7 +202,7 @@ def FLUID_SIGNATURES(fabp, dp, vp):
     }
 
 
-SOLVER_YEE, SOLVER_CKC = 0, 1
+SOLVER_YEE, SOLVER_CKC, SOLVER_NONE = 0, 1, 2
 PIC_ERR_ABORT, PIC_ERR_RETURN = 0, 1
 PUSHER_BORIS, PUSHER_VAY, PUSHER_HC = 0, 1, 2
 # pic_set_deposit_mode / pic_set_gather_mode (include/pic_b200.h)

@@ -64,6 +64,7 @@ struct Species {
     int* bnd_work = nullptr;     // pic_particles_boundary_workspace_ints(bnd_cap) ints, engine-owned
     int bnd_cap = 0;
     bool bins_stale = false;     // particles were removed / the window moved: re-sort before the next step
+    bool bins_exact = false;     // the bins hold every particle's current cell (set by a sort, cleared by a position push)
 };
 
 // Laser antenna: its own particle container (LaserParticleContainer), no gather, order-agnostic deposit
@@ -80,16 +81,23 @@ struct Laser {
 // recorded on the stream the stages are launched on, inside the same pic_engine_evolve calls a benchmark times.
 enum { ST_FILL_EB = 0, ST_GATHER_PUSH, ST_ZERO_J, ST_DEPOSIT, ST_SYNC_J, ST_EVOLVE_B, ST_FILL_B, ST_EVOLVE_E, ST_FILL_E,
        ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_FLUID_GATHER_PUSH, ST_FLUID_FILL,
-       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COUNT };
+       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COLLISIONS, ST_COUNT };
 static const char* const stage_names[ST_COUNT] = {"fill_boundary_eb", "gather_push", "zero_j", "deposit", "sync_current",
     "evolve_b", "fill_boundary_b", "evolve_e", "fill_boundary_e", "wrap", "migrate", "sort", "nci_filter", "move_window", "push_p", "filter_j",
-    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit"};
+    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit", "collisions"};
 // Cold fluid species (WarpXFluidContainer): two borrowed states of N, NUx, NUy, NUz; the advection writes one from the
 // other and `cur` names the current one.
 struct Fluid {
     double q, m;
     pic_fab U[2][4];
     int cur = 0;
+};
+
+// One entry of collisions.collision_names (CollisionHandler): pairwise Coulomb collisions of species isp1 with isp2.
+struct Collision {
+    int isp1, isp2, ndt;
+    double coulomb_log;
+    uint64_t seed;
 };
 
 struct StageRec { int st; cudaEvent_t a, b; };
@@ -145,6 +153,8 @@ struct Engine {
     int* host_count = nullptr;                   // pinned host int (particles lost per boundary pass)
     std::vector<Laser> lasers;
     std::vector<Fluid> fluids;
+    std::vector<Collision> collisions;
+    int* coll_status = nullptr;                  // device int: a cell exceeded the collision kernel's capacity
 };
 
 struct Stage {      // records the events of one stage when timing is on
@@ -386,6 +396,7 @@ static int push(Engine& e, Species& sp, double dt, int push_position, void* s) {
     // particles moved first
     if (!(push_position && sp.has_bins && e.nox <= 3 && g_gather_mode == PIC_GATHER_TILE)) ENG_CALL(apply_pending(sp, s));
     const pic_soa& P = sp.buf[sp.cur];
+    if (push_position) sp.bins_exact = false;
     if (push_position && sp.has_esc) {
         cudaMemsetAsync(sp.esc.count, 0, sizeof(int), (cudaStream_t)s);
         // Over several ranks the push lists what leaves the BRICK (a superset by 1e-6 cell, so that round-off at a face
@@ -437,6 +448,10 @@ static int apply_nci(Engine& e, void* s) {
 }
 
 static int push_particles_and_deposit(Engine& e, void* s) {
+    if (e.solver == PIC_SOLVER_NONE) {       // gather + push with the deposition skipped (WarpXEvolve.cpp:176-182)
+        for (auto& sp : e.species) { Stage t(e, ST_GATHER_PUSH, s); ENG_CALL(push(e, sp, e.dt, 1, s)); }
+        return 0;
+    }
     {
         Stage t(e, ST_ZERO_J, s);
         if (e.use_filter && !e.jdep_alloc) {
@@ -495,6 +510,7 @@ static int sort_species(Engine& e, Species& sp, bool defer, void* s) {
     ENG_CALL(pic_sort_index_by_cell(&in, &e.geom, &sp.bins, sp.sort_work, &sp.pending_src, s));
     sp.bins.np_binned = in.np;
     sp.has_bins = true;
+    sp.bins_exact = true;
     sp.esc_valid = false;
     return defer ? 0 : apply_pending(sp, s);
 }
@@ -701,6 +717,33 @@ static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
     return pic_fluid_deposit_current(fl.U[fl.cur], e.use_filter ? e.jdep : &e.fab[6], fl.q, s);
 }
 
+// MultiParticleContainer::doCollisions -> CollisionHandler::doCollisions (Particles/Collision/CollisionHandler.cpp:85-93)
+// at t_new: a collision runs when int(floor(t / dt)) % ndt == 0, with dt * ndt.  Its species need their current cells:
+// one not sorted since its last position push (or with particles appended behind the bins) is sorted here first, with
+// the move left to this step's gather + push like the end-of-step sort.
+static int do_collisions(Engine& e, void* s) {
+    for (size_t ic = 0; ic < e.collisions.size(); ++ic) {
+        const Collision& c = e.collisions[ic];
+        if (int(std::floor(e.cur_time / e.dt)) % c.ndt != 0) continue;
+        Species* sp[2] = {&e.species[c.isp1], &e.species[c.isp2]};
+        for (Species* p : sp)
+            if (!p->bins_exact || p->bins.np_binned != p->buf[p->cur].np) {
+                Stage t(e, ST_SORT, s);
+                ENG_CALL(sort_species(e, *p, true, s));
+            }
+        Stage t(e, ST_COLLISIONS, s);
+        pic_coulomb_collision cc;
+        cc.q1 = sp[0]->q; cc.m1 = sp[0]->m; cc.q2 = sp[1]->q; cc.m2 = sp[1]->m;
+        cc.coulomb_log = c.coulomb_log; cc.seed = c.seed; cc.collision_index = (int)ic;
+        cc.same_species = c.isp1 == c.isp2 ? 1 : 0;
+        ENG_CALL(pic_collide_pairwise_coulomb(&cc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, sp[0]->pending_src,
+                                              &sp[1]->buf[sp[1]->cur], &sp[1]->bins, sp[1]->pending_src, &e.geom,
+                                              e.dt * c.ndt, e.istep, pic_sort_scratch(sp[0]->sort_work, sp[0]->bins.np_binned),
+                                              pic_sort_scratch(sp[1]->sort_work, sp[1]->bins.np_binned), e.coll_status, s));
+    }
+    return 0;
+}
+
 // last: Synchronize() ends the step; defer_sort: another step of the same call follows, its push moves the sorted particles
 static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     // ---- ExplicitFillBoundaryEBUpdateAux ----
@@ -712,16 +755,20 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
         Stage t(e, ST_FILL_EB, s);
         ENG_CALL(fill_boundary(e, 0, 6, e.ng_FG, s));                    // :515-516
     }
+    // ---- mypc->doCollisions, :157-159 ----
+    if (!e.collisions.empty()) ENG_CALL(do_collisions(e, s));
     // ---- OneStep_nosub ----
     ENG_CALL(push_particles_and_deposit(e, s));
     for (auto& fl : e.fluids) ENG_CALL(evolve_fluid(e, fl, s));      // myfl->Evolve, :1171-1178
-    if (e.use_filter) { Stage t(e, ST_FILTER, s); ENG_CALL(pic_apply_filter_multi(e.jdep, &e.fab[6], 3, e.npass, s)); }
-    { Stage t(e, ST_SYNC_J, s); ENG_CALL(sync_current(e, s)); }
-    { Stage t(e, ST_EVOLVE_B, s); ENG_CALL(evolve_b(e, 0.5 * e.dt, s)); }
-    { Stage t(e, ST_FILL_B, s); ENG_CALL(fill_boundary(e, 3, 6, e.ng_FS, s)); }
-    { Stage t(e, ST_EVOLVE_E, s); ENG_CALL(evolve_e(e, e.dt, s)); }
-    { Stage t(e, ST_FILL_E, s); ENG_CALL(fill_boundary(e, 0, 3, e.ng_FS, s)); }
-    { Stage t(e, ST_EVOLVE_B, s); ENG_CALL(evolve_b(e, 0.5 * e.dt, s)); }
+    if (e.solver != PIC_SOLVER_NONE) {                                    // no J, no field update (:176-182)
+        if (e.use_filter) { Stage t(e, ST_FILTER, s); ENG_CALL(pic_apply_filter_multi(e.jdep, &e.fab[6], 3, e.npass, s)); }
+        { Stage t(e, ST_SYNC_J, s); ENG_CALL(sync_current(e, s)); }
+        { Stage t(e, ST_EVOLVE_B, s); ENG_CALL(evolve_b(e, 0.5 * e.dt, s)); }
+        { Stage t(e, ST_FILL_B, s); ENG_CALL(fill_boundary(e, 3, 6, e.ng_FS, s)); }
+        { Stage t(e, ST_EVOLVE_E, s); ENG_CALL(evolve_e(e, e.dt, s)); }
+        { Stage t(e, ST_FILL_E, s); ENG_CALL(fill_boundary(e, 0, 3, e.ng_FS, s)); }
+        { Stage t(e, ST_EVOLVE_B, s); ENG_CALL(evolve_b(e, 0.5 * e.dt, s)); }
+    }
     if (last) {                                                           // Synchronize(), :64-91
         { Stage t(e, ST_FILL_EB, s); ENG_CALL(fill_boundary(e, 0, 6, e.ng_FG, s)); }
         { Stage t(e, ST_PUSHP, s); for (auto& sp : e.species) ENG_CALL(push(e, sp, 0.5 * e.dt, 0, s)); }
@@ -781,6 +828,8 @@ extern "C" void pic_apply_env_defaults(void) { static EnvDefaults once; (void)on
 extern "C" void* pic_engine_create(const pic_geom* geom, const int box_lo[3], const int box_hi[3], int nox,
                                    int galerkin, int pusher, int solver, double cfl, double dt,
                                    int sort_interval, int use_filter, const int filter_npass[3]) {
+    if (solver == PIC_SOLVER_NONE && !(dt > 0)) { fail("pic_engine_create: algo.maxwell_solver = none needs an explicit dt"); return nullptr; }
+    if (solver == PIC_SOLVER_NONE && use_filter) { fail("pic_engine_create: algo.maxwell_solver = none takes no current filter"); return nullptr; }
     Engine* e = new Engine();
     e->geom = *geom;
     e->use_filter = use_filter ? 1 : 0;
@@ -792,7 +841,8 @@ extern "C" void* pic_engine_create(const pic_geom* geom, const int box_lo[3], co
     }
     e->nox = nox; e->galerkin = galerkin; e->pusher = pusher; e->solver = solver; e->sort_interval = sort_interval;
     e->dt = dt > 0 ? dt : cfl * max_dt(solver, e->dx);
-    stencil_coefficients(solver, e->dx, &e->st);
+    if (solver != PIC_SOLVER_NONE) stencil_coefficients(solver, e->dx, &e->st);
+    else e->st = pic_stencil{};
     guard_cells(*e);
     return e;
 }
@@ -816,6 +866,7 @@ extern "C" void pic_engine_destroy(void* h) {
         if (e->shift_tmp) cudaFree(e->shift_tmp);
         if (e->nci_alloc) for (int c = 0; c < 6; ++c) cudaFree(e->nci_fab[c].p);
         if (e->host_count) cudaFreeHost(e->host_count);
+        if (e->coll_status) cudaFree(e->coll_status);
         for (int b = 0; b < 4; ++b) if (e->hbuf[b]) cudaFree(e->hbuf[b]);
     }
     delete e;
@@ -1051,6 +1102,7 @@ extern "C" int pic_engine_set_boost(void* h, double gamma_boost, double beta_boo
 extern "C" int pic_engine_set_nci_corrector(void* h, const double stencil_exeybz[5], const double stencil_bxbyez[5]) {
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(e->species.empty() && e->lasers.empty(), "pic_engine_set_nci_corrector: call before adding particles");
+    PIC_REQUIRE(e->solver != PIC_SOLVER_NONE, "pic_engine_set_nci_corrector: algo.maxwell_solver = none has no field solver to correct");
     PIC_REQUIRE(e->comm == nullptr, "pic_engine_set_nci_corrector: call before pic_engine_set_comm");
     e->use_nci = true;
     for (int i = 0; i < 5; ++i) { e->nci_stencil[0][i] = stencil_exeybz[i]; e->nci_stencil[1][i] = stencil_bxbyez[i]; }
@@ -1079,6 +1131,7 @@ extern "C" int pic_engine_set_injector(void* h, int isp, const pic_plasma_inject
 extern "C" int pic_engine_add_laser(void* h, const pic_laser_antenna* prm, const pic_soa* p, long capacity) {
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_laser: runs with fluid species take no antennas yet");
+    PIC_REQUIRE(e->solver != PIC_SOLVER_NONE, "pic_engine_add_laser: algo.maxwell_solver = none deposits no current");
     double info[4];
     PIC_REQUIRE(same_boost(*e, prm->gamma_boost, prm->beta_boost), "pic_engine_add_laser: the antenna's gamma_boost / beta_boost differ from pic_engine_set_boost");
     ENG_CALL(pic_laser_antenna_info(prm, e->dx, info));
@@ -1113,10 +1166,44 @@ extern "C" int pic_engine_species_buffer(void* h, int isp, long* np) {
 // WarpX::Evolve(numsteps): the last step synchronises u with x when synchronize_last is set
 extern "C" int pic_engine_evolve(void* h, int numsteps, int synchronize_last, void* stream) {
     Engine* e = static_cast<Engine*>(h);
+    if (!e->collisions.empty()) cudaMemsetAsync(e->coll_status, 0, sizeof(int), (cudaStream_t)stream);
     for (int n = 0; n < numsteps; ++n) {
         const bool final_step = n == numsteps - 1;
         ENG_CALL(one_step(*e, synchronize_last && final_step, !final_step, stream));
     }
+    if (!e->collisions.empty()) {        // one read per call: did a cell exceed the collision kernel's capacity?
+        int st = 0;
+        cudaMemcpyAsync(&st, e->coll_status, sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
+        if (cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+            return fail("pic_engine_evolve: %s", cudaGetErrorString(cudaGetLastError()));
+        PIC_REQUIRE(st == 0, "pic_engine_evolve: a collision found no scratch for a cell of more than 2048 particles");
+    }
+    return 0;
+}
+
+extern "C" int pic_engine_add_collision(void* h, int isp1, int isp2, double coulomb_log, int ndt, uint64_t seed) {
+    Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e, "pic_engine_add_collision: no engine");
+    const int nsp = (int)e->species.size();
+    PIC_REQUIRE(isp1 >= 0 && isp1 < nsp && isp2 >= 0 && isp2 < nsp, "pic_engine_add_collision: no species %d / %d", isp1, isp2);
+    PIC_REQUIRE(ndt >= 1, "pic_engine_add_collision: ndt must be at least 1 (got %d)", ndt);
+    PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_collision: runs with fluid species take no collisions");
+    PIC_REQUIRE(e->comm == nullptr, "pic_engine_add_collision: one rank only (collisions over several ranks are not "
+                                    "yet checked against a single box)");
+    for (int isp : {isp1, isp2}) {
+        const Species& sp = e->species[isp];
+        PIC_REQUIRE(sp.sort_work && sp.bins.cell_start, "pic_engine_add_collision: species %d has no cell bins", isp);
+        for (int d = 0; d < 3; ++d)
+            PIC_REQUIRE(sp.bins.tile[d] == e->species[isp1].bins.tile[d], "pic_engine_add_collision: the species' bins use different tiles");
+    }
+    if (!e->coll_status) {
+        if (cudaMalloc(&e->coll_status, sizeof(int)) != cudaSuccess) {
+            cudaGetLastError();
+            e->coll_status = nullptr;
+            return fail("pic_engine_add_collision: cannot allocate the status word");
+        }
+    }
+    e->collisions.push_back(Collision{isp1, isp2, ndt, coulomb_log, seed});
     return 0;
 }
 
@@ -1133,6 +1220,8 @@ extern "C" int pic_engine_add_fluid_species(void* h, double q, double m, const p
     PIC_REQUIRE(e->comm == nullptr, "pic_engine_add_fluid_species: one rank only");
     PIC_REQUIRE(e->species.empty() && e->lasers.empty(), "pic_engine_add_fluid_species: runs with particle species or antennas take no fluids yet");
     PIC_REQUIRE(m > 0.0, "pic_engine_add_fluid_species: mass must be positive");
+    PIC_REQUIRE(e->solver != PIC_SOLVER_NONE, "pic_engine_add_fluid_species: algo.maxwell_solver = none is not supported");
+    PIC_REQUIRE(e->collisions.empty(), "pic_engine_add_fluid_species: runs with collisions take no fluids");
     for (int b = 0; b < 2; ++b)
         for (int c = 0; c < 4; ++c) {
             const pic_fab& f = (b ? stateB : stateA)[c];

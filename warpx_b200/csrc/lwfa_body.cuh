@@ -17,6 +17,7 @@
 #define PIC_LWFA_BODY_CUH_
 
 #include "pic_common.cuh"
+#include "philox.cuh"
 
 namespace pic {
 
@@ -277,29 +278,7 @@ PIC_HD bool boundary_body(long ip, const BoundaryArgs& a) {          // returns 
 // Gaussian beam (AddGaussianBeam, PhysicalParticleContainer.cpp:503-677).  The reference draws from AMReX's
 // per-thread stream; here draw i takes the counter-based Philox4x64-10 blocks 2i and 2i+1, so that every
 // decomposition (and the numpy reference, warpx_b200.workloads.beam_normals) sees the same draws.
-// Philox4x64-10 of Random123 (Salmon et al., SC'11): 10 rounds, multipliers M0/M1, Weyl key increments W0/W1.
-// Block j = the output of numpy.random.Philox(key=seed) after advance(j): counter (j + 1, 0, 0, 0), key (seed, 0).
-PIC_HD uint64_t mulhi64(uint64_t a, uint64_t b) {
-#ifdef __CUDA_ARCH__
-    return __umul64hi(a, b);
-#else
-    return (uint64_t)(((unsigned __int128)a * b) >> 64);
-#endif
-}
-
-PIC_HD void philox4x64_10(uint64_t seed, uint64_t block, uint64_t out[4]) {
-    const uint64_t M0 = 0xD2E7470EE14C6C93ull, M1 = 0xCA5A826395121157ull;
-    const uint64_t W0 = 0x9E3779B97F4A7C15ull, W1 = 0xBB67AE8584CAA73Bull;
-    uint64_t c0 = block + 1, c1 = 0, c2 = 0, c3 = 0, k0 = seed, k1 = 0;
-    for (int r = 0; r < 10; ++r) {
-        if (r > 0) { k0 += W0; k1 += W1; }
-        const uint64_t hi0 = mulhi64(M0, c0), lo0 = M0 * c0;
-        const uint64_t hi1 = mulhi64(M1, c2), lo1 = M1 * c2;
-        const uint64_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-        c0 = n0; c1 = lo1; c2 = n2; c3 = lo0;
-    }
-    out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
+// Block j = the output of numpy.random.Philox(key=seed) after advance(j): philox4x64_10 of philox.cuh.
 
 // Four normals of one block, as workloads.philox_normal forms them: 53-bit uniforms u in [0, 1), radii from
 // u1 = 1 - u of words 0 and 1, angles 2 pi u of words 2 and 3: (r0 cos, r0 sin, r1 cos, r1 sin).

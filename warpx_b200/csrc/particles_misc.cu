@@ -284,6 +284,12 @@ extern "C" int pic_sort_index_by_cell(const pic_soa* in, const pic_geom* g, cons
     return check_launch("pic_sort_index_by_cell") ? 0 : 1;
 }
 
+// the per-particle int array of the sort workspace that only pic_sort_index_by_cell uses (its bin keys): free between
+// sorts, np entries for the np of the last index
+extern "C" int* pic_sort_scratch(void* work, long np) {
+    return reinterpret_cast<int*>(static_cast<char*>(work) + align256((size_t)np * 4));
+}
+
 extern "C" int pic_sort_apply_permutation(const pic_soa* in, const pic_soa* out, const int* src, void* stream) {
     const long np = in->np;
     PIC_REQUIRE(out->np == np, "pic_sort_apply_permutation: in/out sizes differ");

@@ -134,7 +134,7 @@ def write_plotfile(sim, prefix, iteration=None, fields=("Ex", "Ey", "Ez", "Bx", 
         with open(os.path.join(root, "warpx_job_info"), "w") as f:
             f.write("=" * 78 + "\n warpx_b200 job information\n" + "=" * 78 + "\n")
             f.write("number of ranks (one per GPU): %d\nparticle shape order: %d\nsolver: %s\n"
-                    % (world, sim.nox, "CKC" if sim.solver == abi.SOLVER_CKC else "Yee"))
+                    % (world, sim.nox, {abi.SOLVER_CKC: "CKC", abi.SOLVER_NONE: "none"}.get(sim.solver, "Yee")))
     # ---- particles ----
     which = range(len(sim.species)) if species is None else species
     for isp in which:

@@ -215,8 +215,12 @@ class Simulation:
         """boundaries: abi.pic_boundaries (boundary.field_lo/hi, boundary.particle_lo/hi; default all
         periodic); moving_window: (direction, v/c) == warpx.do_moving_window / moving_window_dir /
         moving_window_v; nb: brick grid (default parallel.brick_grid(world); a moving window needs slabs
-        along its direction, e.g. (1, 1, world)); use_bins=False: no cell sort, the order-agnostic kernels."""
+        along its direction, e.g. (1, 1, world)); use_bins=False: no cell sort, the order-agnostic kernels.
+        solver=abi.SOLVER_NONE (algo.maxwell_solver = none): the fields are never updated, the particles are gathered
+        and pushed without depositing; it needs an explicit dt and takes no filter, antenna, NCI corrector or fluid."""
         global _error_source
+        if solver == abi.SOLVER_NONE and not dt:
+            raise ValueError("algo.maxwell_solver = none needs an explicit dt")
         self.torch, self.L, self.device = self._backend(device)
         _error_source = self.L
         t = self.torch
@@ -273,6 +277,9 @@ class Simulation:
         self.native = self.L.pic_engine_create(C.byref(self.geom), abi.int3(self.box_lo), abi.int3(self.box_hi),
                                                nox, galerkin, pusher, solver, cfl, self.dt, sort_interval,
                                                1 if self.use_filter else 0, abi.int3(self.filter_npass))
+        if not self.native:
+            raise RuntimeError("pic_b200: " + self.L.pic_last_error().decode())
+        self.collisions = []
         if boundaries is not None:
             check(self.L.pic_engine_set_boundaries(self.native, C.byref(boundaries)))
         if moving_window is not None:
@@ -460,6 +467,26 @@ class Simulation:
         check(self.L.pic_engine_add_laser(self.native, C.byref(laser), C.byref(soa), max(n, 1)))
         self.lasers.append(dict(laser=laser, buf=buf, ids=ids, np=n))
         return len(self.lasers) - 1
+
+    def add_collision(self, species1, species2, coulomb_log=-1.0, ndt=1, seed=0):
+        """One entry of collisions.collision_names with <name>.type = pairwisecoulomb: <name>.species = species1
+        species2 (Species objects, names or indices; the same species twice is an intra-species collision),
+        <name>.CoulombLog (<= 0: computed per pair from the cell's Debye length) and <name>.ndt.  seed keys the
+        collision's random streams (warpx.random_seed): a run's result depends on the particles by id, the seed, the
+        collision's position in the list, the step and the cell, not on their storage order.  One rank only.  A restarted run registers
+        its collisions again, in the same order.  Returns the collision's index."""
+        isp = [self._species_index(v) for v in (species1, species2)]
+        check(self.L.pic_engine_add_collision(self.native, isp[0], isp[1], float(coulomb_log), int(ndt), int(seed)))
+        self.collisions.append(dict(species=tuple(isp), coulomb_log=float(coulomb_log), ndt=int(ndt), seed=int(seed)))
+        return len(self.collisions) - 1
+
+    def _species_index(self, v):
+        if isinstance(v, (int, np.integer)):
+            return int(v)
+        for i, sp in enumerate(self.species):
+            if sp is v or (isinstance(v, str) and sp.name == v):
+                return i
+        raise ValueError("add_collision: no species %r" % (v,))
 
     def laser_numpy(self, il, sort_by_id=True):
         la = self.lasers[il]

@@ -96,6 +96,7 @@ def bind(L):
         "pic_sort_particles_by_cell": (C.c_int, [soap, soap, gp, bp, vp, vp]),
         "pic_sort_index_by_cell": (C.c_int, [soap, gp, bp, vp, C.POINTER(vp), vp]),
         "pic_sort_apply_permutation": (C.c_int, [soap, soap, vp, vp]),
+        "pic_sort_scratch": (vp, [vp, C.c_long]),
         "pic_sum_squares_unique": (C.c_int, [fabp, gp, vp, vp]),
         "pic_particle_energy": (C.c_int, [soap, C.c_double, vp, vp]),
         "pic_engine_create": (vp, [gp, ip, ip, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int,
@@ -131,6 +132,7 @@ def bind(L):
     }
     sig.update(abi.LWFA_SIGNATURES(fabp, soap, gp, bndp, lasp, injp, dp, ip, vp))
     sig.update(abi.FLUID_SIGNATURES(fabp, dp, vp))
+    sig.update(abi.COLLISION_SIGNATURES(soap, bp, gp, vp))
     for name, (res, args) in sig.items():
         fn = getattr(L, name)      # AttributeError if include/pic_b200.h and the library disagree
         fn.restype = res

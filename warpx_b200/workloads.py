@@ -179,6 +179,59 @@ def uniform_plasma_3d(n=256, ppc=(2, 2, 2), lx=40.0e-6, density=1.0e25, u_th=0.0
     return dict(n_cell=n_cell, prob_lo=prob_lo, prob_hi=prob_hi, species=species)
 
 
+def _random_per_cell(seed, n_cell, prob_lo, prob_hi, ppc):
+    """NRandomPerCell: ppc positions uniform inside every cell (cell i fastest, then j, k; the particles of a cell
+    consecutive).  Particle p takes Philox4x64-10 block p of `seed` (philox_blocks), words 0-2 as 53-bit uniforms."""
+    n_cell = np.asarray(n_cell)
+    dx = (np.asarray(prob_hi, dtype=np.float64) - np.asarray(prob_lo, dtype=np.float64)) / n_cell
+    ncell = int(np.prod(n_cell))
+    K, J, I = np.meshgrid(*[np.arange(n_cell[d]) for d in (2, 1, 0)], indexing="ij")
+    cells = [np.repeat(a.ravel(), ppc) for a in (I, J, K)]
+    u = (philox_blocks(seed, 0, ncell * ppc)[:, :3] >> np.uint64(11)).astype(np.float64) * (1.0 / 9007199254740992.0)
+    return [np.ascontiguousarray(prob_lo[d] + (cells[d] + u[:, d]) * dx[d]) for d in range(3)]
+
+
+def _collision_species(name, q, m, seed, n_cell, prob_lo, prob_hi, ppc, density, u_th, u_m=(0.0, 0.0, 0.0)):
+    """momentum_distribution_type = "gaussian": u = (u_m + u_th N(0, 1)) c per component (philox_normal of seed + 1)"""
+    x, y, z = _random_per_cell(seed, n_cell, prob_lo, prob_hi, ppc)
+    dV = np.prod((np.asarray(prob_hi) - np.asarray(prob_lo)) / np.asarray(n_cell))
+    g = philox_normal(seed + 1, 0, len(x))
+    u = [np.ascontiguousarray((u_m[d] + u_th[d] * g[:, d]) * C) for d in range(3)]
+    return dict(name=name, q=q, m=m, x=x, y=y, z=z, w=np.full(len(x), density * dV / ppc), ux=u[0], uy=u[1], uz=u[2])
+
+
+def collision_xyz_3d(n=8, ppc=200, seed=2034958209):
+    """Examples/Tests/collision/inputs_test_3d_collision_xyz: electrons and ions (mass 5 m_e, the deck's value) at
+    1e21 m^-3, 200 random particles per cell each, electrons drifting along x; algo.maxwell_solver = none, dt =
+    1.224744871e-07, 150 steps; electron-ion, electron-electron and ion-ion collisions with CoulombLog 15.9 every 10
+    steps.  n: cells per axis (the deck's 8; other values keep its cell size); seed: warpx.random_seed."""
+    lx = 4.154046151855669e2 * n / 8
+    n_cell, prob_lo, prob_hi = (n,) * 3, (0.0,) * 3, (lx,) * 3
+    ue, ui = 0.044237441120300, 0.006256118919701
+    species = [_collision_species("electron", -Q_E, M_E, seed, n_cell, prob_lo, prob_hi, ppc, 1.0e21, (ue,) * 3, (ue, 0, 0)),
+               _collision_species("ion", Q_E, 4.554691780000000e-30, seed + 2, n_cell, prob_lo, prob_hi, ppc, 1.0e21,
+                                  (ui,) * 3)]
+    collisions = [dict(species=(0, 1), coulomb_log=15.9, ndt=10, seed=seed),
+                  dict(species=(0, 0), coulomb_log=15.9, ndt=10, seed=seed),
+                  dict(species=(1, 1), coulomb_log=15.9, ndt=10, seed=seed)]
+    # analysis_collision_3d.py: <ux_e - ux_i>/c ~ a exp(b step) at steps 0, 10, ..., 150, mean error < 0.001
+    return dict(n_cell=n_cell, prob_lo=prob_lo, prob_hi=prob_hi, dt=1.224744871e-07, max_step=150, species=species,
+                collisions=collisions, analysis=dict(a=0.041817463099883, b=-0.083851393560288, tolerance=0.001))
+
+
+def collision_iso_3d(n=8, ppc=1000, seed=1):
+    """Examples/Tests/collision/inputs_test_3d_collision_iso: electrons at 1.116e28 m^-3, 1000 random particles per
+    cell, anisotropic temperature (u_th 0.0033163 c along x, 0.0031592 c across); algo.maxwell_solver = none, dt =
+    1.4e-17, 100 steps (stop_time 1.4e-15); electron-electron collisions with CoulombLog 2 every step."""
+    lx = 4.0e-6 * n / 8
+    n_cell, prob_lo, prob_hi = (n,) * 3, (0.0,) * 3, (lx,) * 3
+    u_th = (0.0033163331635535603, 0.00315918518549115, 0.00315918518549115)
+    species = [_collision_species("electron", -Q_E, M_E, seed, n_cell, prob_lo, prob_hi, ppc, 1.116e28, u_th)]
+    return dict(n_cell=n_cell, prob_lo=prob_lo, prob_hi=prob_hi, dt=1.4e-17, max_step=100, species=species,
+                collisions=[dict(species=(0, 0), coulomb_log=2.0, ndt=1, seed=seed)],
+                analysis=dict(T_par=5.62, T_per=5.1, ne=1.116e28, coulomb_log=2.0, tolerance=0.05))
+
+
 def laser_acceleration_3d(n_cell=(32, 32, 256), max_step=100, solver=0, pusher=0):
     """Config 4's deterministic ancestor: Examples/Physics_applications/laser_acceleration/
     inputs_base_3d (test_3d_laser_acceleration): Yee, Boris, order 3, bilinear filter on (WarpX
