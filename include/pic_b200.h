@@ -697,9 +697,83 @@ int pic_collide_pairwise_coulomb(const pic_coulomb_collision* c, const pic_soa* 
  * <name>.ndt >= 1, the random seed.  Collisions run after ExplicitFillBoundaryEBUpdateAux and before the push
  * (WarpXEvolve.cpp:141-159), at the steps with int(floor(t / dt)) % ndt == 0, with dt * ndt.  A colliding species is
  * sorted by cell before its collision whenever its bins are stale.  Species without bins, indices out of range,
- * ndt < 1, runs with fluid species and runs over several ranks (not yet checked against a single box) are refused
- * before the engine changes. */
+ * ndt < 1, runs with fluid species, runs over several ranks (not yet checked against a single box) and a species that
+ * is a reactant of an earlier pic_engine_add_fusion entry are refused before the engine changes. */
 int pic_engine_add_collision(void* engine, int isp1, int isp2, double coulomb_log, int ndt, uint64_t seed);
+
+/* ------------------------------------------------------------------------------------------
+ * Two-product nuclear fusion (collisions.collision_names, <name>.type = nuclearfusion), 3D Cartesian:
+ * NuclearFusionFunc (Source/Particles/Collision/BinaryCollision/NuclearFusion/NuclearFusionFunc.H) with
+ * SingleNuclearFusionEvent.H, BoschHaleFusionCrossSection.H and the products of ParticleCreationFunc.H:205-225
+ * (TwoProductFusionInitializeMomentum.H).  Proton-boron and D + He3 are not supported.
+ * ---------------------------------------------------------------------------------------- */
+enum { PIC_FUSION_DT_NHE4 = 0,   /* D + T  -> n + He4, 17.5893 MeV   (DeuteriumTritiumToNeutronHelium)  */
+       PIC_FUSION_DD_PT = 1,     /* D + D  -> p + T,   4.032667 MeV  (DeuteriumDeuteriumToProtonTritium) */
+       PIC_FUSION_DD_NHE3 = 2 }; /* D + D  -> n + He3, 3.268911 MeV  (DeuteriumDeuteriumToNeutronHelium) */
+
+/* Particle id of a reactant whose weight the fusion used up (BinaryCollisionUtils.H:140-162 sets
+ * amrex::ParticleIdCpus::Invalid): later pairs skip it, later fusion entries of the step leave it out (the engine refuses
+ * a Coulomb entry that would follow a fusion on a shared species), and the step removes it
+ * where it removes the particles lost at absorbing faces. */
+#define PIC_SPENT_ID 0xFFFFFFFFFFFFFFFFull
+
+typedef struct pic_fusion_collision {
+    double q1, m1, q2, m2;       /* reactants 1 and 2 (species 2 = species 1 when same_species)              */
+    double mA, mB;               /* product species A and B, in the order of <name>.product_species          */
+    int type;                    /* PIC_FUSION_*                                                             */
+    double fusion_multiplier;                /* <name>.fusion_multiplier (default 1)                        */
+    double fusion_probability_threshold;     /* <name>.fusion_probability_threshold (default 0.02)          */
+    double fusion_probability_target_value;  /* <name>.fusion_probability_target_value (default 0.002)      */
+    uint64_t seed;               /* key of the Philox4x64-10 streams                                         */
+    int collision_index;         /* position in collisions.collision_names                                   */
+    int same_species;
+} pic_fusion_collision;
+
+/* Device workspace of one fusion collision whose reactants hold at most np1 + np2 particles (np1 when same_species)
+ * over `nbins` bins: per-pair records at the cell's own slots, per-bin pair and event counts, their scan. */
+long pic_fusion_workspace_bytes(long pair_capacity, long nbins);
+
+/* The event pass: BinaryCollision::doCollisionsWithinTile (BinaryCollision/BinaryCollision.H:383-472 intra-species,
+ * :613-730 inter-species) with NuclearFusionFunc::Executor (NuclearFusionFunc.H:127-234) over the box of the bins, dt =
+ * the collision's dt.  Per cell: the live particles (id != PIC_SPENT_ID) of each species in ascending id order,
+ * ShuffleFisherYates, the pair chains with SingleNuclearFusionEvent; an event takes w_min / multiplier_eff from both
+ * reactants and marks a reactant left with weight <= DBL_MIN spent.  Only w and ids change.  The pairs and the
+ * per-bin event counts go to `work` (pic_fusion_workspace_bytes(pair_capacity, bins)) for
+ * pic_fusion_create_products.  Bins, permutations, scratch and *status as for pic_collide_pairwise_coulomb. */
+int pic_collide_nuclear_fusion(const pic_fusion_collision* c, const pic_soa* p1, const pic_bins* b1, const int* src1,
+                               const pic_soa* p2, const pic_bins* b2, const int* src2, const pic_geom* g, double dt,
+                               long step, int* scratch1, int* scratch2, void* work, long pair_capacity, int* status,
+                               void* stream);
+
+/* The product pass (ParticleCreationFunc.H:120-230 with TwoProductFusionInitializeMomentum): an exclusive scan of the
+ * event counts, ONE host read of the total (synchronises `stream`), then event e of the call -- cell-major, pair order
+ * inside the cell -- writes product A at slots pA->np + 2e, + 1 and product B at pB->np + 2e, + 1: the first of each
+ * pair at reactant 1's position, the second at reactant 2's, weight w / 2, ids next_id + 2e (+ 1), momenta isotropic
+ * in the centre-of-momentum frame.  The reactants and bins are those of the event pass, unchanged since.  *n_events
+ * receives the number of events; the caller adds 2 n_events to both products' counts.  When a product would exceed
+ * its capacity nothing is written and the call fails naming the product and the capacity needed. */
+int pic_fusion_create_products(const pic_fusion_collision* c, const pic_soa* p1, const pic_bins* b1, const pic_soa* p2,
+                               const pic_bins* b2, const pic_geom* g, long step, void* work, long pair_capacity,
+                               const pic_soa* pA, long capA, uint64_t next_idA, const pic_soa* pB, long capB,
+                               uint64_t next_idB, long* n_events, void* stream);
+
+/* Lists the particles whose id is PIC_SPENT_ID for pic_particles_boundary_compact: work and cap as for
+ * pic_particles_boundary_mark, work[0] = how many. */
+int pic_particles_mark_spent(const pic_soa* p, int* work, int cap, void* stream);
+
+/* One fusion entry of collisions.collision_names for the step driver: reactants isp1, isp2 (the same index:
+ * intra-species), products iprodA, iprodB (PIC_FUSION_* order), type, multiplier, probability threshold and target,
+ * ndt, seed.  It shares the collision index and the schedule of pic_engine_add_collision.  The event pass runs in the
+ * `fusion` stage, the product pass in `fusion_products`; the spent reactants are removed in the step's particle
+ * boundary stage.  Refused before the engine changes: indices out of range, reactants without bins, a product equal
+ * to a reactant or to the other product, ndt < 1, a bad type or parameter, fluid species, several ranks. */
+int pic_engine_add_fusion(void* engine, int isp1, int isp2, int iprodA, int iprodB, int type, double multiplier,
+                          double probability_threshold, double probability_target_value, int ndt, uint64_t seed);
+/* The id counter of species isp: the id the next particle it creates receives (fusion products; ids next_id, next_id
+ * + 1, ...).  It starts at the species' initial particle count; a checkpoint carries it.  The setter refuses a value
+ * below the species' current count. */
+uint64_t pic_engine_species_next_id(void* engine, int isp);
+int pic_engine_set_species_next_id(void* engine, int isp, uint64_t next_id);
 
 /* Number of kernels launched by this library since load (bench.py's gpu_launches). */
 long pic_launch_count(void);

@@ -83,6 +83,16 @@ class pic_coulomb_collision(C.Structure):
                 ("same_species", C.c_int)]
 
 
+class pic_fusion_collision(C.Structure):
+    _fields_ = [("q1", C.c_double), ("m1", C.c_double), ("q2", C.c_double), ("m2", C.c_double),
+                ("mA", C.c_double), ("mB", C.c_double), ("type", C.c_int), ("fusion_multiplier", C.c_double),
+                ("fusion_probability_threshold", C.c_double), ("fusion_probability_target_value", C.c_double),
+                ("seed", C.c_uint64), ("collision_index", C.c_int), ("same_species", C.c_int)]
+
+
+FUSION_DT_NHE4, FUSION_DD_PT, FUSION_DD_NHE3 = 0, 1, 2
+SPENT_ID = 0xFFFFFFFFFFFFFFFF          # PIC_SPENT_ID: a reactant whose weight a fusion used up
+
 FIELD_PERIODIC, FIELD_PEC = 0, 1
 PARTICLE_PERIODIC, PARTICLE_ABSORBING, PARTICLE_REFLECTING = 0, 1, 2
 _FIELD_BC = {"periodic": FIELD_PERIODIC, "pec": FIELD_PEC}
@@ -187,6 +197,17 @@ def COLLISION_SIGNATURES(soap, bp, gp, vp):
         "pic_collide_pairwise_coulomb": (C.c_int, [C.POINTER(pic_coulomb_collision), soap, bp, vp, soap, bp, vp, gp,
                                                    C.c_double, C.c_long, vp, vp, vp, vp]),
         "pic_engine_add_collision": (C.c_int, [vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_uint64]),
+        "pic_fusion_workspace_bytes": (C.c_long, [C.c_long, C.c_long]),
+        "pic_collide_nuclear_fusion": (C.c_int, [C.POINTER(pic_fusion_collision), soap, bp, vp, soap, bp, vp, gp,
+                                                 C.c_double, C.c_long, vp, vp, vp, C.c_long, vp, vp]),
+        "pic_fusion_create_products": (C.c_int, [C.POINTER(pic_fusion_collision), soap, bp, soap, bp, gp, C.c_long, vp,
+                                                 C.c_long, soap, C.c_long, C.c_uint64, soap, C.c_long, C.c_uint64,
+                                                 C.POINTER(C.c_long), vp]),
+        "pic_particles_mark_spent": (C.c_int, [soap, vp, C.c_int, vp]),
+        "pic_engine_species_next_id": (C.c_uint64, [vp, C.c_int]),
+        "pic_engine_set_species_next_id": (C.c_int, [vp, C.c_int, C.c_uint64]),
+        "pic_engine_add_fusion": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
+                                            C.c_double, C.c_int, C.c_uint64]),
     }
 
 

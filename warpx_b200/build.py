@@ -12,9 +12,9 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
          "-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
-# The fluid and collision kernels restate the reference's arithmetic operation by operation: no multiply-add
+# The fluid, collision and fusion kernels restate the reference's arithmetic operation by operation: no multiply-add
 # contraction there.
-FILE_FLAGS = {"fluid.cu": ["-fmad=false"], "collision.cu": ["-fmad=false"]}
+FILE_FLAGS = {"fluid.cu": ["-fmad=false"], "collision.cu": ["-fmad=false"], "fusion.cu": ["-fmad=false"]}
 
 
 def sources():

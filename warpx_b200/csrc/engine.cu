@@ -65,6 +65,9 @@ struct Species {
     int bnd_cap = 0;
     bool bins_stale = false;     // particles were removed / the window moved: re-sort before the next step
     bool bins_exact = false;     // the bins hold every particle's current cell (set by a sort, cleared by a position push)
+    // fusion reactant: the particles a fusion spent (id PIC_SPENT_ID) are listed here for the compaction, capacity + 1
+    int* spent_work = nullptr;
+    int spent_cap = 0;
 };
 
 // Laser antenna: its own particle container (LaserParticleContainer), no gather, order-agnostic deposit
@@ -81,10 +84,10 @@ struct Laser {
 // recorded on the stream the stages are launched on, inside the same pic_engine_evolve calls a benchmark times.
 enum { ST_FILL_EB = 0, ST_GATHER_PUSH, ST_ZERO_J, ST_DEPOSIT, ST_SYNC_J, ST_EVOLVE_B, ST_FILL_B, ST_EVOLVE_E, ST_FILL_E,
        ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_FLUID_GATHER_PUSH, ST_FLUID_FILL,
-       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COLLISIONS, ST_COUNT };
+       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COLLISIONS, ST_FUSION, ST_FUSION_PRODUCTS, ST_COUNT };
 static const char* const stage_names[ST_COUNT] = {"fill_boundary_eb", "gather_push", "zero_j", "deposit", "sync_current",
     "evolve_b", "fill_boundary_b", "evolve_e", "fill_boundary_e", "wrap", "migrate", "sort", "nci_filter", "move_window", "push_p", "filter_j",
-    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit", "collisions"};
+    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit", "collisions", "fusion", "fusion_products"};
 // Cold fluid species (WarpXFluidContainer): two borrowed states of N, NUx, NUy, NUz; the advection writes one from the
 // other and `cur` names the current one.
 struct Fluid {
@@ -93,11 +96,18 @@ struct Fluid {
     int cur = 0;
 };
 
-// One entry of collisions.collision_names (CollisionHandler): pairwise Coulomb collisions of species isp1 with isp2.
+// One entry of collisions.collision_names (CollisionHandler): pairwise Coulomb collisions of species isp1 with isp2, or
+// (fusion) nuclear fusion of isp1 with isp2 into iprod[0], iprod[1] with its engine-owned pair workspace.
 struct Collision {
     int isp1, isp2, ndt;
     double coulomb_log;
     uint64_t seed;
+    bool fusion = false;
+    int iprod[2] = {-1, -1};
+    int type = 0;
+    double multiplier = 1.0, threshold = 0.02, target = 0.002;
+    void* work = nullptr;
+    long pair_cap = 0;
 };
 
 struct StageRec { int st; cudaEvent_t a, b; };
@@ -721,6 +731,37 @@ static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
 // at t_new: a collision runs when int(floor(t / dt)) % ndt == 0, with dt * ndt.  Its species need their current cells:
 // one not sorted since its last position push (or with particles appended behind the bins) is sorted here first, with
 // the move left to this step's gather + push like the end-of-step sort.
+static int do_fusion(Engine& e, const Collision& c, int ic, Species* sp[2], void* s) {
+    pic_fusion_collision fc;
+    fc.q1 = sp[0]->q; fc.m1 = sp[0]->m; fc.q2 = sp[1]->q; fc.m2 = sp[1]->m;
+    Species* pr[2] = {&e.species[c.iprod[0]], &e.species[c.iprod[1]]};
+    fc.mA = pr[0]->m; fc.mB = pr[1]->m;
+    fc.type = c.type; fc.fusion_multiplier = c.multiplier;
+    fc.fusion_probability_threshold = c.threshold; fc.fusion_probability_target_value = c.target;
+    fc.seed = c.seed; fc.collision_index = ic; fc.same_species = c.isp1 == c.isp2 ? 1 : 0;
+    {
+        Stage t(e, ST_FUSION, s);
+        ENG_CALL(pic_collide_nuclear_fusion(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, sp[0]->pending_src,
+                                            &sp[1]->buf[sp[1]->cur], &sp[1]->bins, sp[1]->pending_src, &e.geom,
+                                            e.dt * c.ndt, e.istep, pic_sort_scratch(sp[0]->sort_work, sp[0]->bins.np_binned),
+                                            pic_sort_scratch(sp[1]->sort_work, sp[1]->bins.np_binned), c.work, c.pair_cap,
+                                            e.coll_status, s));
+    }
+    Stage t(e, ST_FUSION_PRODUCTS, s);
+    for (Species* p : pr) ENG_CALL(apply_pending(*p, s));       // products are appended behind the particles in place
+    long nev = 0;
+    ENG_CALL(pic_fusion_create_products(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, &sp[1]->buf[sp[1]->cur],
+                                        &sp[1]->bins, &e.geom, e.istep, c.work, c.pair_cap, &pr[0]->buf[pr[0]->cur],
+                                        pr[0]->capacity, pr[0]->next_id, &pr[1]->buf[pr[1]->cur], pr[1]->capacity,
+                                        pr[1]->next_id, &nev, s));
+    for (Species* p : pr) {
+        p->buf[p->cur].np += 2 * nev;
+        p->next_id += (uint64_t)(2 * nev);
+        if (nev) p->bins_stale = true;
+    }
+    return 0;
+}
+
 static int do_collisions(Engine& e, void* s) {
     for (size_t ic = 0; ic < e.collisions.size(); ++ic) {
         const Collision& c = e.collisions[ic];
@@ -731,6 +772,7 @@ static int do_collisions(Engine& e, void* s) {
                 Stage t(e, ST_SORT, s);
                 ENG_CALL(sort_species(e, *p, true, s));
             }
+        if (c.fusion) { ENG_CALL(do_fusion(e, c, (int)ic, sp, s)); continue; }
         Stage t(e, ST_COLLISIONS, s);
         pic_coulomb_collision cc;
         cc.q1 = sp[0]->q; cc.m1 = sp[0]->m; cc.q2 = sp[1]->q; cc.m2 = sp[1]->m;
@@ -740,6 +782,32 @@ static int do_collisions(Engine& e, void* s) {
                                               &sp[1]->buf[sp[1]->cur], &sp[1]->bins, sp[1]->pending_src, &e.geom,
                                               e.dt * c.ndt, e.istep, pic_sort_scratch(sp[0]->sort_work, sp[0]->bins.np_binned),
                                               pic_sort_scratch(sp[1]->sort_work, sp[1]->bins.np_binned), e.coll_status, s));
+    }
+    return 0;
+}
+
+// The reactants a fusion spent leave with the particles lost at the boundaries (the reference's
+// deleteInvalidParticles, BinaryCollision.H:212-218): all marks, ONE host read of the counts, the compactions.
+static int remove_spent(Engine& e, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    bool any = false;
+    for (size_t n = 0; n < e.species.size(); ++n) {
+        Species& sp = e.species[n];
+        if (!sp.spent_work) continue;
+        ENG_CALL(apply_pending(sp, s));
+        ENG_CALL(pic_particles_mark_spent(&sp.buf[sp.cur], sp.spent_work, sp.spent_cap, s));
+        cudaMemcpyAsync(e.host_count + n, sp.spent_work, sizeof(int), cudaMemcpyDeviceToHost, s);
+        any = true;
+    }
+    if (!any) return 0;
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail("pic_engine: spent-reactant pass failed (%s)", cudaGetErrorString(cudaGetLastError()));
+    for (size_t n = 0; n < e.species.size(); ++n) {
+        Species& sp = e.species[n];
+        if (!sp.spent_work || e.host_count[n] == 0) continue;
+        pic_soa& P = sp.buf[sp.cur];
+        ENG_CALL(pic_particles_boundary_compact(&P, sp.spent_work, sp.spent_cap, e.host_count[n], s));
+        P.np -= e.host_count[n];
+        sp.bins_stale = true;
     }
     return 0;
 }
@@ -791,6 +859,7 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
         }
         for (auto& L : e.lasers) ENG_CALL(pic_particles_wrap_periodic(&L.P, &e.geom, s));
         ENG_CALL(apply_particle_boundaries(e, s));
+        ENG_CALL(remove_spent(e, s));
     }
     for (auto& sp : e.species) {
         if (e.comm) { Stage t(e, ST_MIGRATE, s); ENG_CALL(migrate(e, sp, s)); }
@@ -861,12 +930,14 @@ extern "C" void pic_engine_destroy(void* h) {
             if (sp.mig_work) cudaFree(sp.mig_work);
             if (sp.mig_head) cudaFreeHost(sp.mig_head);
             if (sp.bnd_work) cudaFree(sp.bnd_work);
+            if (sp.spent_work) cudaFree(sp.spent_work);
         }
         for (auto& L : e->lasers) { if (L.bnd_work) cudaFree(L.bnd_work); if (L.w_owned) cudaFree(L.w_owned); }
         if (e->shift_tmp) cudaFree(e->shift_tmp);
         if (e->nci_alloc) for (int c = 0; c < 6; ++c) cudaFree(e->nci_fab[c].p);
         if (e->host_count) cudaFreeHost(e->host_count);
         if (e->coll_status) cudaFree(e->coll_status);
+        for (auto& c : e->collisions) if (c.work) cudaFree(c.work);
         for (int b = 0; b < 4; ++b) if (e->hbuf[b]) cudaFree(e->hbuf[b]);
     }
     delete e;
@@ -920,6 +991,7 @@ extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa
     PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_species: runs with fluid species take no particle species yet");
     Species sp;
     sp.capacity = capacity;
+    sp.next_id = (uint64_t)bufA->np;     // ids of particles created later (fusion products) follow the initial ones
     sp.q = q; sp.m = m; sp.buf[0] = *bufA; sp.buf[1] = *bufB; sp.cur = 0; sp.has_bins = false; sp.sort_work = sort_work;
     sp.bins.cell_start = cell_start;
     for (int d = 0; d < 3; ++d) sp.bins.tile[d] = tile ? tile[d] : 8;
@@ -1203,6 +1275,12 @@ extern "C" int pic_engine_add_collision(void* h, int isp1, int isp2, double coul
             return fail("pic_engine_add_collision: cannot allocate the status word");
         }
     }
+    // a Coulomb entry after a fusion on one of its species would meet the reactants that fusion spent in the same step
+    // (they leave at the end of the step); the reference removes them between the two collisions
+    for (const Collision& c : e->collisions)
+        PIC_REQUIRE(!c.fusion || (c.isp1 != isp1 && c.isp1 != isp2 && c.isp2 != isp1 && c.isp2 != isp2),
+                    "pic_engine_add_collision: species %d / %d are reactants of an earlier fusion entry; register the "
+                    "Coulomb collision before the fusion", isp1, isp2);
     e->collisions.push_back(Collision{isp1, isp2, ndt, coulomb_log, seed});
     return 0;
 }
@@ -1240,4 +1318,75 @@ extern "C" int pic_engine_add_fluid_species(void* h, double q, double m, const p
 extern "C" int pic_engine_fluid_state(void* h, int i) {
     Engine* e = static_cast<Engine*>(h);
     return (i >= 0 && i < (int)e->fluids.size()) ? e->fluids[i].cur : -1;
+}
+
+// One nuclearfusion entry of collisions.collision_names: see include/pic_b200.h.  Every precondition is checked before
+// the engine changes; the pair workspace and the removal lists of the reactants are allocated here.
+extern "C" int pic_engine_add_fusion(void* h, int isp1, int isp2, int iprodA, int iprodB, int type, double multiplier,
+                                     double probability_threshold, double probability_target_value, int ndt, uint64_t seed) {
+    Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e, "pic_engine_add_fusion: no engine");
+    const int nsp = (int)e->species.size();
+    for (int i : {isp1, isp2, iprodA, iprodB})
+        PIC_REQUIRE(i >= 0 && i < nsp, "pic_engine_add_fusion: no species %d", i);
+    PIC_REQUIRE(iprodA != iprodB, "pic_engine_add_fusion: the two products must be different species");
+    for (int i : {iprodA, iprodB})
+        PIC_REQUIRE(i != isp1 && i != isp2, "pic_engine_add_fusion: a product species (%d) cannot be a reactant", i);
+    PIC_REQUIRE(type == PIC_FUSION_DT_NHE4 || type == PIC_FUSION_DD_PT || type == PIC_FUSION_DD_NHE3,
+                "pic_engine_add_fusion: unknown fusion type %d", type);
+    PIC_REQUIRE(multiplier > 0.0 && probability_threshold > 0.0 && probability_target_value > 0.0,
+                "pic_engine_add_fusion: the multiplier, threshold and target value must be positive");
+    PIC_REQUIRE(ndt >= 1, "pic_engine_add_fusion: ndt must be at least 1 (got %d)", ndt);
+    PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_fusion: runs with fluid species take no collisions");
+    PIC_REQUIRE(e->comm == nullptr, "pic_engine_add_fusion: one rank only (collisions over several ranks are not "
+                                    "yet checked against a single box)");
+    for (int isp : {isp1, isp2}) {
+        const Species& sp = e->species[isp];
+        PIC_REQUIRE(sp.sort_work && sp.bins.cell_start, "pic_engine_add_fusion: species %d has no cell bins", isp);
+        for (int d = 0; d < 3; ++d)
+            PIC_REQUIRE(sp.bins.tile[d] == e->species[isp1].bins.tile[d], "pic_engine_add_fusion: the species' bins use different tiles");
+    }
+    Collision c{isp1, isp2, ndt, 0.0, seed};
+    c.fusion = true; c.iprod[0] = iprodA; c.iprod[1] = iprodB; c.type = type;
+    c.multiplier = multiplier; c.threshold = probability_threshold; c.target = probability_target_value;
+    c.pair_cap = e->species[isp1].capacity + (isp1 == isp2 ? 0 : e->species[isp2].capacity);
+    const long nbins = pic_bins_count(e->box_lo, e->box_hi, e->species[isp1].bins.tile);
+    bool ok = cudaMalloc(&c.work, (size_t)pic_fusion_workspace_bytes(c.pair_cap, nbins)) == cudaSuccess;
+    if (ok && !e->coll_status) ok = cudaMalloc(&e->coll_status, sizeof(int)) == cudaSuccess;
+    int* spent[2] = {nullptr, nullptr};
+    for (int k = 0; k < 2 && ok; ++k) {
+        const Species& sp = e->species[k ? isp2 : isp1];
+        if (sp.spent_work || (k == 1 && isp1 == isp2)) continue;
+        ok = cudaMalloc(&spent[k], sizeof(int) * (size_t)pic_particles_boundary_workspace_ints((int)(sp.capacity + 1))) == cudaSuccess;
+    }
+    if (!ok) {
+        cudaGetLastError();
+        if (c.work) cudaFree(c.work);
+        for (int* p : spent) if (p) cudaFree(p);
+        return fail("pic_engine_add_fusion: cannot allocate the fusion workspace");
+    }
+    for (int k = 0; k < 2; ++k)
+        if (spent[k]) {
+            Species& sp = e->species[k ? isp2 : isp1];
+            sp.spent_work = spent[k];
+            sp.spent_cap = (int)(sp.capacity + 1);
+        }
+    e->collisions.push_back(c);
+    return 0;
+}
+
+// The id the next particle species isp creates (fusion products, injected plasma) receives; a restart sets it from the
+// checkpoint so that new ids never repeat old ones.  The setter refuses a counter below the species' particle count.
+extern "C" uint64_t pic_engine_species_next_id(void* h, int isp) {
+    Engine* e = static_cast<Engine*>(h);
+    return (e && isp >= 0 && isp < (int)e->species.size()) ? e->species[isp].next_id : 0;
+}
+extern "C" int pic_engine_set_species_next_id(void* h, int isp, uint64_t next_id) {
+    Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e && isp >= 0 && isp < (int)e->species.size(), "pic_engine_set_species_next_id: no species %d", isp);
+    Species& sp = e->species[isp];
+    PIC_REQUIRE(next_id >= (uint64_t)sp.buf[sp.cur].np, "pic_engine_set_species_next_id: %llu is below the %ld particles",
+                (unsigned long long)next_id, (long)sp.buf[sp.cur].np);
+    sp.next_id = next_id;
+    return 0;
 }

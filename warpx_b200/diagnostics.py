@@ -226,7 +226,7 @@ def write_checkpoint(sim, prefix, iteration=None, file_min_digits=5):
             f.write(")\n")
             f.write("%d\n" % len(sim.species))
             for sp in sim.species:
-                f.write("%s %.17g %.17g\n" % (sp.name, sp.q, sp.m))
+                f.write("%s %.17g %.17g%s\n" % (sp.name, sp.q, sp.m, " " + sp.species_type if sp.species_type else ""))
     for isp, sp in enumerate(sim.species):
         sdir = os.path.join(root, sp.name, "Level_0")
         if rank == 0:
@@ -247,8 +247,11 @@ def write_checkpoint(sim, prefix, iteration=None, file_min_digits=5):
         counts = _gather(sim, [float(n)])
         if rank == 0:
             ntot = int(sum(c[0] for c in counts))
+            # the next-id field, 1-based as AMReX's ids: the species' id counter + 1 (at least ntot + 1); fusion products
+            # continue from it after a restart
+            next_id = max(ntot, sim.species_next_id(isp)) + 1 if sim.world == 1 else ntot + 1
             with open(os.path.join(root, sp.name, "Header"), "w") as f:
-                f.write("Version_Two_Dot_Zero_double\n3\n4\nw\nux\nuy\nuz\n0\n1\n%d\n%d\n0\n%d\n" % (ntot, ntot + 1, world))
+                f.write("Version_Two_Dot_Zero_double\n3\n4\nw\nux\nuy\nuz\n0\n1\n%d\n%d\n0\n%d\n" % (ntot, next_id, world))
                 for r in range(world):
                     f.write("%d %d 0\n" % (r, int(counts[r][0])))
     if sim.dist is not None and world > 1:
@@ -256,9 +259,12 @@ def write_checkpoint(sim, prefix, iteration=None, file_min_digits=5):
     return root
 
 
-def read_checkpoint(sim, root):
+def read_checkpoint(sim, root, capacity=None):
     """Load a checkpoint written by write_checkpoint into a freshly constructed Simulation with the same grid, guard
-    cells and decomposition and no species yet: fields with guards, the species with their ids, step counter and time."""
+    cells and decomposition and no species yet: fields with guards, the species with their ids, species types and id
+    counters, step counter and time.  capacity: {species name: entries of its particle arrays} for species that must
+    grow after the restart (e.g. fusion products); the others get room for their particles only.  Collisions and
+    fusion entries are registered again afterwards, in the same order."""
     with open(os.path.join(root, "WarpXHeader")) as f:
         h = [ln.strip() for ln in f]
     assert h[0] == "Checkpoint version: 1" and int(h[1]) == 1
@@ -279,7 +285,7 @@ def read_checkpoint(sim, root):
         a = np.fromfile(path, dtype="<f8")
         assert a.size == sim.data[c].numel(), "guard cells of the restart differ from the checkpoint's (%s)" % CHK_FIELDS[c]
         sim.data[c].copy_(t.from_numpy(a.reshape(tuple(sim.data[c].shape))))
-    for name, q, m in species:
+    for isp, (name, q, m, *stype) in enumerate(species):
         with open(os.path.join(root, name, "Header")) as f:
             ph = [ln.strip() for ln in f]
         assert ph[0] == "Version_Two_Dot_Zero_double" and int(ph[8]) == 1      # is_checkpoint
@@ -293,7 +299,11 @@ def read_checkpoint(sim, root):
             ints = np.frombuffer(f.read(8 * count), dtype="<i4").reshape(count, 2)
             rec = np.frombuffer(f.read(56 * count), dtype="<f8").reshape(count, 7)
         ids = (ints[:, 0].astype(np.int64) & 0xFFFFFFFF) | (ints[:, 1].astype(np.int64) << 32)
-        sim.add_species(name, float(q), float(m), *[np.ascontiguousarray(rec[:, k]) for k in range(7)], ids=ids)
+        sim.add_species(name, float(q), float(m), *[np.ascontiguousarray(rec[:, k]) for k in range(7)], ids=ids,
+                        species_type=stype[0] if stype else None,
+                        capacity=(capacity or {}).get(name))
+        if sim.world == 1 and int(ph[10]) - 1 > count:
+            sim.set_species_next_id(isp, int(ph[10]) - 1)
     sim.set_step(istep, time)
     sim.is_synchronized = True
     return istep

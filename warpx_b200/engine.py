@@ -143,9 +143,10 @@ def release_comm(dist):
 class Species:
     NAMES = ("x", "y", "z", "w", "ux", "uy", "uz")
 
-    def __init__(self, sim, name, q, m, arrays, capacity, ids=None):
+    def __init__(self, sim, name, q, m, arrays, capacity, ids=None, species_type=None):
         t = sim.torch
         self.sim, self.name, self.q, self.m = weakref.proxy(sim), name, q, m
+        self.species_type = canonical_species_type(species_type) if species_type is not None else None
         self.np = len(arrays["x"])
         self.capacity = max(capacity, self.np)
         # two SoA buffers: the counting sort permutes from one into the other
@@ -178,6 +179,52 @@ class Species:
 
     def array(self, name):
         return self.buf[self.cur][self.NAMES.index(name), :self.np]
+
+
+# <species>.species_type -> (charge [C], mass [kg]): Source/Particles/SpeciesPhysicalProperties.cpp, with its aliases
+Q_E, M_P, M_U = 1.602176634e-19, 1.67262192369e-27, 1.66053906660e-27    # PhysConst::q_e, m_p, m_u
+_SPECIES_ALIASES = {"protium": "hydrogen1", "deuterium": "hydrogen2", "tritium": "hydrogen3"}
+SPECIES_PROPERTIES = {
+    "neutron": (0.0, 1.0013784193052508 * M_P),
+    "proton": (Q_E, M_P),
+    "hydrogen1": (1 * Q_E, 1.00782503223 * M_U),
+    "hydrogen2": (1 * Q_E, 2.01410177812 * M_U),
+    "hydrogen3": (1 * Q_E, 3.0160492779 * M_U),
+    "helium3": (2 * Q_E, 3.0160293201 * M_U),
+    "helium4": (2 * Q_E, 4.00260325413 * M_U),
+}
+
+
+def canonical_species_type(name):
+    """The table's name of a species_type (aliases resolved); unknown names are refused."""
+    k = _SPECIES_ALIASES.get(str(name).lower(), str(name).lower())
+    if k not in SPECIES_PROPERTIES:
+        raise ValueError("unknown species_type %r (known: %s)" % (name, ", ".join(sorted(set(SPECIES_PROPERTIES) | set(_SPECIES_ALIASES)))))
+    return k
+
+
+def species_charge_mass(species_type):
+    """(q, m) of a species_type, as <species>.species_type sets them."""
+    return SPECIES_PROPERTIES[canonical_species_type(species_type)]
+
+
+def nuclear_fusion_type(reactants, products):
+    """BinaryCollisionUtils::get_nuclear_fusion_type (BinaryCollisionUtils.cpp:40-123) for the two-product reactions:
+    the abi.FUSION_* of the reactants' and products' species types; other combinations are refused."""
+    r, p = sorted(reactants), sorted(products)
+    if r == ["hydrogen2", "hydrogen3"]:
+        if p != ["helium4", "neutron"]:
+            raise ValueError("deuterium-tritium fusion: the products must be of type neutron and helium4")
+        return abi.FUSION_DT_NHE4
+    if r == ["hydrogen2", "hydrogen2"]:
+        if p == ["helium3", "neutron"]:
+            return abi.FUSION_DD_NHE3
+        if p == ["hydrogen1", "hydrogen3"]:
+            return abi.FUSION_DD_PT
+        raise ValueError("deuterium-deuterium fusion: the products must be of type helium3 and neutron, or hydrogen3 and "
+                         "hydrogen1")
+    raise NotImplementedError("nuclear fusion between species of type %s and %s is not supported (D + T and D + D only)"
+                              % tuple(reactants))
 
 
 class FluidSpecies:
@@ -344,27 +391,42 @@ class Simulation:
     def stream(self):
         return self.torch.cuda.current_stream().cuda_stream
 
-    def add_species(self, name, q, m, x, y, z, w, ux, uy, uz, capacity_factor=None, ids=None):
+    def add_species(self, name, q, m, x, y, z, w, ux, uy, uz, capacity_factor=None, ids=None, species_type=None,
+                    capacity=None):
         """Particles must lie inside this rank's box (use workloads.* with box_lo/box_hi).  ids: 64-bit particle ids
-        (default: rank << 40 | index)."""
+        (default: rank << 40 | index).  species_type: <species>.species_type (see SPECIES_PROPERTIES), which
+        add_fusion reads.  capacity: entries of every particle array (default len(x) * capacity_factor); a species that
+        receives fusion products needs room for them."""
         if capacity_factor is None:
             capacity_factor = 1.0 if self.world == 1 else 1.25
         if self.fluids:
             raise NotImplementedError("runs with fluid species take no particle species")
         arrays = dict(x=x, y=y, z=z, w=w, ux=ux, uy=uy, uz=uz)
-        cap = int(len(x) * capacity_factor) + (0 if self.world == 1 else 65536)
-        sp = Species(self, name, q, m, arrays, cap, ids=ids)
+        cap = int(len(x) * capacity_factor) + (0 if self.world == 1 else 65536) if capacity is None else int(capacity)
+        sp = Species(self, name, q, m, arrays, cap, ids=ids, species_type=species_type)
         self._register_species(sp)
         return sp
 
-    def add_plasma_species(self, name, q, m, injector, capacity):
+    def add_empty_species(self, name, capacity, species_type=None, q=None, m=None):
+        """A species without particles and room for `capacity` (e.g. the products of a fusion).  q and m default to
+        those of species_type."""
+        if species_type is not None:
+            dq, dm = species_charge_mass(species_type)
+            q, m = dq if q is None else q, dm if m is None else m
+        if q is None or m is None:
+            raise ValueError("add_empty_species: give species_type or q and m")
+        empty = np.empty(0)
+        return self.add_species(name, q, m, empty, empty, empty, empty, empty, empty, empty, species_type=species_type,
+                                capacity=int(capacity))
+
+    def add_plasma_species(self, name, q, m, injector, capacity, species_type=None):
         """A species created on the device by its plasma injector (PhysicalParticleContainer::InitData ->
         AddPlasma over the whole domain, PhysicalParticleContainer.cpp:450-454,855-922); with
         injector.do_continuous_injection the moving window keeps refilling the uncovered slab.
-        capacity: entries of every particle array (the run must never exceed it)."""
+        capacity: entries of every particle array (the run must never exceed it).  species_type: as for add_species."""
         injector.gamma_boost, injector.beta_boost = self.gamma_boost, self.beta_boost
         empty = np.empty(0)
-        sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity))
+        sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity), species_type=species_type)
         soa = sp.soa(0)
         # ids = creation index in the order a single box would create the particles (k slowest): the
         # ranks below this one come first when the bricks are slabs along z
@@ -387,15 +449,16 @@ class Simulation:
         check(self.L.pic_engine_set_injector(self.native, len(self.species) - 1, C.byref(injector)))
         return sp
 
-    def add_beam_species(self, name, q, m, beam, capacity):
+    def add_beam_species(self, name, q, m, beam, capacity, species_type=None):
         """A Gaussian beam (abi.pic_gaussian_beam, <species>.injection_style = "gaussian_beam") created on the device by
         pic_add_gaussian_beam (PhysicalParticleContainer::AddGaussianBeam + InitData, PhysicalParticleContainer.cpp:
         450-454,503-677), in the lab frame or mapped into this run's boosted frame at the current time.  Each rank keeps
         the particles of its own brick; ids are creation indices, the same on any decomposition.  A beam is created
-        once and never refilled.  capacity: entries of every particle array (the run must never exceed it)."""
+        once and never refilled.  capacity: entries of every particle array (the run must never exceed it).  species_type:
+        as for add_species."""
         beam.gamma_boost, beam.beta_boost = self.gamma_boost, self.beta_boost
         empty = np.empty(0)
-        sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity))
+        sp = Species(self, name, q, m, {k: empty for k in Species.NAMES}, int(capacity), species_type=species_type)
         soa = sp.soa(0)
         # this brick's half-open share of the domain; the domain's own faces are open (the library drops or wraps there)
         own_lo = [self.prob_lo[d] + self.dx[d] * self.box_lo[d] if self.box_lo[d] > 0 else -math.inf for d in range(3)]
@@ -479,6 +542,40 @@ class Simulation:
         check(self.L.pic_engine_add_collision(self.native, isp[0], isp[1], float(coulomb_log), int(ndt), int(seed)))
         self.collisions.append(dict(species=tuple(isp), coulomb_log=float(coulomb_log), ndt=int(ndt), seed=int(seed)))
         return len(self.collisions) - 1
+
+    def add_fusion(self, species1, species2, products, multiplier=1.0, probability_threshold=0.02,
+                   probability_target_value=0.002, ndt=1, seed=0):
+        """One entry of collisions.collision_names with <name>.type = nuclearfusion: <name>.species = species1 species2
+        (the same species twice: D + D within one species), <name>.product_species = products (two species, in the
+        order the products are written), <name>.fusion_multiplier, fusion_probability_threshold,
+        fusion_probability_target_value and ndt.  The reaction follows from the species types, as
+        get_nuclear_fusion_type infers it: D + T -> n + He4, D + D -> n + He3 or p + T.  Products appear at their
+        reactants' positions; reactants whose weight is used up leave the run at the end of the step.  It shares the
+        collision index, the schedule and the determinism of add_collision.  One rank only.  Returns the index."""
+        isp = [self._species_index(v) for v in (species1, species2)]
+        if len(products) != 2:
+            raise ValueError("add_fusion: a two-product fusion takes exactly two product species")
+        ipr = [self._species_index(v) for v in products]
+        types = [self.species[i].species_type for i in isp + ipr]
+        if any(v is None for v in types):
+            raise ValueError("add_fusion: every reactant and product needs a species_type")
+        ftype = nuclear_fusion_type(types[:2], types[2:])
+        check(self.L.pic_engine_add_fusion(self.native, isp[0], isp[1], ipr[0], ipr[1], ftype, float(multiplier),
+                                           float(probability_threshold), float(probability_target_value), int(ndt),
+                                           int(seed)))
+        self.collisions.append(dict(species=tuple(isp), products=tuple(ipr), type=ftype, multiplier=float(multiplier),
+                                    probability_threshold=float(probability_threshold),
+                                    probability_target_value=float(probability_target_value), ndt=int(ndt),
+                                    seed=int(seed)))
+        return len(self.collisions) - 1
+
+    def species_next_id(self, isp):
+        """The id the next particle species isp creates receives (its id counter)."""
+        return int(self.L.pic_engine_species_next_id(self.native, int(isp)))
+
+    def set_species_next_id(self, isp, next_id):
+        """Restart: continue species isp's id counter from a checkpoint."""
+        check(self.L.pic_engine_set_species_next_id(self.native, int(isp), int(next_id)))
 
     def _species_index(self, v):
         if isinstance(v, (int, np.integer)):
@@ -577,6 +674,20 @@ class Simulation:
             self.dist.all_reduce(out)
         v = out.cpu().numpy()
         return [(float(v[i, 0]), float(v[i, 1])) for i in range(len(self.species))]
+
+    def particle_number(self):
+        """ParticleNumber reduced diagnostic (Diagnostics/ReducedDiags/ParticleNumber.cpp): per species (number of
+        macroparticles, sum of weights), summed over ranks."""
+        out = []
+        for sp in self.species:
+            w = sp.array("w")
+            n, ws = sp.np, float(w.sum().item()) if sp.np else 0.0
+            if self.dist is not None and self.world > 1:
+                tt = self.torch.tensor([float(n), ws], dtype=self.torch.float64, device=self.device)
+                self.dist.all_reduce(tt)
+                n, ws = int(tt[0].item()), float(tt[1].item())
+            out.append((int(n), ws))
+        return out
 
     def rho_numpy(self):
         """The `rho` diagnostic of a plotfile (Diagnostics/ComputeDiagFunctors/RhoFunctor.cpp:35-81): every
