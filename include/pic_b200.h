@@ -702,14 +702,17 @@ int pic_collide_pairwise_coulomb(const pic_coulomb_collision* c, const pic_soa* 
 int pic_engine_add_collision(void* engine, int isp1, int isp2, double coulomb_log, int ndt, uint64_t seed);
 
 /* ------------------------------------------------------------------------------------------
- * Two-product nuclear fusion (collisions.collision_names, <name>.type = nuclearfusion), 3D Cartesian:
+ * Nuclear fusion (collisions.collision_names, <name>.type = nuclearfusion), 3D Cartesian:
  * NuclearFusionFunc (Source/Particles/Collision/BinaryCollision/NuclearFusion/NuclearFusionFunc.H) with
- * SingleNuclearFusionEvent.H, BoschHaleFusionCrossSection.H and the products of ParticleCreationFunc.H:205-225
- * (TwoProductFusionInitializeMomentum.H).  Proton-boron and D + He3 are not supported.
+ * SingleNuclearFusionEvent.H, BoschHaleFusionCrossSection.H or ProtonBoronFusionCrossSection.H, and the products of
+ * ParticleCreationFunc.H:170-225 (TwoProductFusionInitializeMomentum.H, ProtonBoronFusionInitializeMomentum.H).
+ * D + He3 is not supported.
  * ---------------------------------------------------------------------------------------- */
 enum { PIC_FUSION_DT_NHE4 = 0,   /* D + T  -> n + He4, 17.5893 MeV   (DeuteriumTritiumToNeutronHelium)  */
        PIC_FUSION_DD_PT = 1,     /* D + D  -> p + T,   4.032667 MeV  (DeuteriumDeuteriumToProtonTritium) */
-       PIC_FUSION_DD_NHE3 = 2 }; /* D + D  -> n + He3, 3.268911 MeV  (DeuteriumDeuteriumToNeutronHelium) */
+       PIC_FUSION_DD_NHE3 = 2,   /* D + D  -> n + He3, 3.268911 MeV  (DeuteriumDeuteriumToNeutronHelium) */
+       PIC_FUSION_PB_3HE4 = 3 }; /* p + B11 -> 3 He4 through alpha + 8Be*, 5.55610759 + 3.12600414 MeV
+                                  * (ProtonBoronToAlphas); one product species, mB unused */
 
 /* Particle id of a reactant whose weight the fusion used up (BinaryCollisionUtils.H:140-162 sets
  * amrex::ParticleIdCpus::Invalid): later pairs skip it, later fusion entries of the step leave it out (the engine refuses
@@ -751,7 +754,11 @@ int pic_collide_nuclear_fusion(const pic_fusion_collision* c, const pic_soa* p1,
  * pair at reactant 1's position, the second at reactant 2's, weight w / 2, ids next_id + 2e (+ 1), momenta isotropic
  * in the centre-of-momentum frame.  The reactants and bins are those of the event pass, unchanged since.  *n_events
  * receives the number of events; the caller adds 2 n_events to both products' counts.  When a product would exceed
- * its capacity nothing is written and the call fails naming the product and the capacity needed. */
+ * its capacity nothing is written and the call fails naming the product and the capacity needed.
+ * PIC_FUSION_PB_3HE4 (ParticleCreationFunc.H:170-200 with ProtonBoronFusionInitializeMomentum): pB may be NULL and
+ * is not touched; event e writes six alphas into pA: alpha k = 0, 1, 2 at slots pA->np + 6e + 2k (reactant 1's
+ * position) and + 1 (reactant 2's), weight w / 2, ids next_idA + 6e + 2k (+ 1), the two of each k with one momentum;
+ * the caller adds 6 n_events to pA's count. */
 int pic_fusion_create_products(const pic_fusion_collision* c, const pic_soa* p1, const pic_bins* b1, const pic_soa* p2,
                                const pic_bins* b2, const pic_geom* g, long step, void* work, long pair_capacity,
                                const pic_soa* pA, long capA, uint64_t next_idA, const pic_soa* pB, long capB,
@@ -762,7 +769,8 @@ int pic_fusion_create_products(const pic_fusion_collision* c, const pic_soa* p1,
 int pic_particles_mark_spent(const pic_soa* p, int* work, int cap, void* stream);
 
 /* One fusion entry of collisions.collision_names for the step driver: reactants isp1, isp2 (the same index:
- * intra-species), products iprodA, iprodB (PIC_FUSION_* order), type, multiplier, probability threshold and target,
+ * intra-species), products iprodA, iprodB (PIC_FUSION_* order; iprodB = -1 for PIC_FUSION_PB_3HE4 and only for it,
+ * whose alphas all go to iprodA), type, multiplier, probability threshold and target,
  * ndt, seed.  It shares the collision index and the schedule of pic_engine_add_collision.  The event pass runs in the
  * `fusion` stage, the product pass in `fusion_products`; the spent reactants are removed in the step's particle
  * boundary stage.  Refused before the engine changes: indices out of range, reactants without bins, a product equal
@@ -774,6 +782,16 @@ int pic_engine_add_fusion(void* engine, int isp1, int isp2, int iprodA, int ipro
  * below the species' current count. */
 uint64_t pic_engine_species_next_id(void* engine, int isp);
 int pic_engine_set_species_next_id(void* engine, int isp, uint64_t next_id);
+
+/* <species>.do_not_push / <species>.do_not_deposit of species isp for the step driver (0 or 1 each; both 0 is the
+ * default).  do_not_push replaces the early returns of WarpXParticleContainer::PushX (WarpXParticleContainer.cpp:1478)
+ * and PhysicalParticleContainer::PushP (PhysicalParticleContainer.cpp:2375) and the skipped gather + push of
+ * PhysicalParticleContainer::Evolve (:1948-2053): the species' positions and momenta keep their bits, in the main
+ * push, in the half pushes of u at the start and end of a run, and with algo.maxwell_solver = none; it is still sorted,
+ * collided, fused and wrapped.  do_not_deposit replaces the early return of DepositCurrent
+ * (WarpXParticleContainer.cpp:370): the species is pushed but adds nothing to J (Simulation.rho_numpy leaves it out
+ * as MultiParticleContainer::GetChargeDensity does, MultiParticleContainer.cpp:576,598).  A bad index is refused. */
+int pic_engine_set_species_flags(void* engine, int isp, int do_not_push, int do_not_deposit);
 
 /* Number of kernels launched by this library since load (bench.py's gpu_launches). */
 long pic_launch_count(void);

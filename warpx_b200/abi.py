@@ -90,7 +90,7 @@ class pic_fusion_collision(C.Structure):
                 ("seed", C.c_uint64), ("collision_index", C.c_int), ("same_species", C.c_int)]
 
 
-FUSION_DT_NHE4, FUSION_DD_PT, FUSION_DD_NHE3 = 0, 1, 2
+FUSION_DT_NHE4, FUSION_DD_PT, FUSION_DD_NHE3, FUSION_PB_3HE4 = 0, 1, 2, 3
 SPENT_ID = 0xFFFFFFFFFFFFFFFF          # PIC_SPENT_ID: a reactant whose weight a fusion used up
 
 FIELD_PERIODIC, FIELD_PEC = 0, 1
@@ -206,6 +206,7 @@ def COLLISION_SIGNATURES(soap, bp, gp, vp):
         "pic_particles_mark_spent": (C.c_int, [soap, vp, C.c_int, vp]),
         "pic_engine_species_next_id": (C.c_uint64, [vp, C.c_int]),
         "pic_engine_set_species_next_id": (C.c_int, [vp, C.c_int, C.c_uint64]),
+        "pic_engine_set_species_flags": (C.c_int, [vp, C.c_int, C.c_int, C.c_int]),
         "pic_engine_add_fusion": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
                                             C.c_double, C.c_int, C.c_uint64]),
     }

@@ -68,6 +68,8 @@ struct Species {
     // fusion reactant: the particles a fusion spent (id PIC_SPENT_ID) are listed here for the compaction, capacity + 1
     int* spent_work = nullptr;
     int spent_cap = 0;
+    bool do_not_push = false;      // <species>.do_not_push: x and u keep their bits (pic_engine_set_species_flags)
+    bool do_not_deposit = false;   // <species>.do_not_deposit: no current deposition
 };
 
 // Laser antenna: its own particle container (LaserParticleContainer), no gather, order-agnostic deposit
@@ -97,7 +99,8 @@ struct Fluid {
 };
 
 // One entry of collisions.collision_names (CollisionHandler): pairwise Coulomb collisions of species isp1 with isp2, or
-// (fusion) nuclear fusion of isp1 with isp2 into iprod[0], iprod[1] with its engine-owned pair workspace.
+// (fusion) nuclear fusion of isp1 with isp2 into iprod[0], iprod[1] (-1 for proton-boron: one product species) with
+// its engine-owned pair workspace.
 struct Collision {
     int isp1, isp2, ndt;
     double coulomb_log;
@@ -457,9 +460,23 @@ static int apply_nci(Engine& e, void* s) {
     return 0;
 }
 
+// A species that is not pushed (do_not_push): the move a deferred sort left out happens here instead of in the gather
+// + push, and its escape list is empty -- nothing left the domain or the brick.  Its bins stay exact.
+static int hold(Species& sp, void* s) {
+    ENG_CALL(apply_pending(sp, s));
+    if (sp.has_esc) {
+        cudaMemsetAsync(sp.esc.count, 0, sizeof(int), (cudaStream_t)s);
+        sp.esc_valid = true;
+    }
+    return 0;
+}
+
 static int push_particles_and_deposit(Engine& e, void* s) {
     if (e.solver == PIC_SOLVER_NONE) {       // gather + push with the deposition skipped (WarpXEvolve.cpp:176-182)
-        for (auto& sp : e.species) { Stage t(e, ST_GATHER_PUSH, s); ENG_CALL(push(e, sp, e.dt, 1, s)); }
+        for (auto& sp : e.species) {
+            Stage t(e, ST_GATHER_PUSH, s);
+            ENG_CALL(sp.do_not_push ? hold(sp, s) : push(e, sp, e.dt, 1, s));
+        }
         return 0;
     }
     {
@@ -482,7 +499,8 @@ static int push_particles_and_deposit(Engine& e, void* s) {
     lower_corner(e, e.ng_J, xyzmin, lo);
     if (e.use_nci && !e.species.empty()) { Stage t(e, ST_NCI, s); ENG_CALL(apply_nci(e, s)); }
     for (auto& sp : e.species) {
-        { Stage t(e, ST_GATHER_PUSH, s); ENG_CALL(push(e, sp, e.dt, 1, s)); }
+        { Stage t(e, ST_GATHER_PUSH, s); ENG_CALL(sp.do_not_push ? hold(sp, s) : push(e, sp, e.dt, 1, s)); }
+        if (sp.do_not_deposit) continue;     // DepositCurrent returns early (WarpXParticleContainer.cpp:370)
         const pic_soa& P = sp.buf[sp.cur];
         Stage t(e, ST_DEPOSIT, s);
         ENG_CALL(pic_deposit_esirkepov(&P, 0, P.np, Jd, e.dinv, xyzmin, lo, sp.q, e.dt, -0.5 * e.dt,
@@ -734,8 +752,9 @@ static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
 static int do_fusion(Engine& e, const Collision& c, int ic, Species* sp[2], void* s) {
     pic_fusion_collision fc;
     fc.q1 = sp[0]->q; fc.m1 = sp[0]->m; fc.q2 = sp[1]->q; fc.m2 = sp[1]->m;
-    Species* pr[2] = {&e.species[c.iprod[0]], &e.species[c.iprod[1]]};
-    fc.mA = pr[0]->m; fc.mB = pr[1]->m;
+    const bool pb = c.type == PIC_FUSION_PB_3HE4;      // one product species: six alphas per event
+    Species* pr[2] = {&e.species[c.iprod[0]], pb ? nullptr : &e.species[c.iprod[1]]};
+    fc.mA = pr[0]->m; fc.mB = pb ? 0.0 : pr[1]->m;
     fc.type = c.type; fc.fusion_multiplier = c.multiplier;
     fc.fusion_probability_threshold = c.threshold; fc.fusion_probability_target_value = c.target;
     fc.seed = c.seed; fc.collision_index = ic; fc.same_species = c.isp1 == c.isp2 ? 1 : 0;
@@ -748,15 +767,18 @@ static int do_fusion(Engine& e, const Collision& c, int ic, Species* sp[2], void
                                             e.coll_status, s));
     }
     Stage t(e, ST_FUSION_PRODUCTS, s);
-    for (Species* p : pr) ENG_CALL(apply_pending(*p, s));       // products are appended behind the particles in place
+    for (Species* p : pr)                // products are appended behind the particles in place
+        if (p) ENG_CALL(apply_pending(*p, s));
     long nev = 0;
     ENG_CALL(pic_fusion_create_products(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, &sp[1]->buf[sp[1]->cur],
                                         &sp[1]->bins, &e.geom, e.istep, c.work, c.pair_cap, &pr[0]->buf[pr[0]->cur],
-                                        pr[0]->capacity, pr[0]->next_id, &pr[1]->buf[pr[1]->cur], pr[1]->capacity,
-                                        pr[1]->next_id, &nev, s));
+                                        pr[0]->capacity, pr[0]->next_id, pb ? nullptr : &pr[1]->buf[pr[1]->cur],
+                                        pb ? 0 : pr[1]->capacity, pb ? 0 : pr[1]->next_id, &nev, s));
+    const long per_event = pb ? 6 : 2;
     for (Species* p : pr) {
-        p->buf[p->cur].np += 2 * nev;
-        p->next_id += (uint64_t)(2 * nev);
+        if (!p) continue;
+        p->buf[p->cur].np += per_event * nev;
+        p->next_id += (uint64_t)(per_event * nev);
         if (nev) p->bins_stale = true;
     }
     return 0;
@@ -817,7 +839,10 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     // ---- ExplicitFillBoundaryEBUpdateAux ----
     if (e.is_synchronized) {
         { Stage t(e, ST_FILL_EB, s); ENG_CALL(fill_boundary(e, 0, 6, e.ng_EB, s)); }                    // ng_alloc_EB, :487-488
-        { Stage t(e, ST_PUSHP, s); for (auto& sp : e.species) ENG_CALL(push(e, sp, -0.5 * e.dt, 0, s)); }   // PushP(-dt/2), :492-504
+        {                                                                 // PushP(-dt/2), :492-504
+            Stage t(e, ST_PUSHP, s);
+            for (auto& sp : e.species) if (!sp.do_not_push) ENG_CALL(push(e, sp, -0.5 * e.dt, 0, s));
+        }
         e.is_synchronized = false;
     } else {
         Stage t(e, ST_FILL_EB, s);
@@ -839,7 +864,10 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     }
     if (last) {                                                           // Synchronize(), :64-91
         { Stage t(e, ST_FILL_EB, s); ENG_CALL(fill_boundary(e, 0, 6, e.ng_FG, s)); }
-        { Stage t(e, ST_PUSHP, s); for (auto& sp : e.species) ENG_CALL(push(e, sp, 0.5 * e.dt, 0, s)); }
+        {
+            Stage t(e, ST_PUSHP, s);
+            for (auto& sp : e.species) if (!sp.do_not_push) ENG_CALL(push(e, sp, 0.5 * e.dt, 0, s));
+        }
         e.is_synchronized = true;
     }
     const long step = e.istep++;
@@ -1327,13 +1355,17 @@ extern "C" int pic_engine_add_fusion(void* h, int isp1, int isp2, int iprodA, in
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(e, "pic_engine_add_fusion: no engine");
     const int nsp = (int)e->species.size();
+    PIC_REQUIRE(type == PIC_FUSION_DT_NHE4 || type == PIC_FUSION_DD_PT || type == PIC_FUSION_DD_NHE3 ||
+                type == PIC_FUSION_PB_3HE4, "pic_engine_add_fusion: unknown fusion type %d", type);
+    const bool pb = type == PIC_FUSION_PB_3HE4;         // one product species
+    PIC_REQUIRE(pb == (iprodB == -1),
+                pb ? "pic_engine_add_fusion: proton-boron fusion takes one product species (iprodB = -1)"
+                   : "pic_engine_add_fusion: this reaction takes two product species");
     for (int i : {isp1, isp2, iprodA, iprodB})
-        PIC_REQUIRE(i >= 0 && i < nsp, "pic_engine_add_fusion: no species %d", i);
+        PIC_REQUIRE((pb && i == iprodB) || (i >= 0 && i < nsp), "pic_engine_add_fusion: no species %d", i);
     PIC_REQUIRE(iprodA != iprodB, "pic_engine_add_fusion: the two products must be different species");
     for (int i : {iprodA, iprodB})
         PIC_REQUIRE(i != isp1 && i != isp2, "pic_engine_add_fusion: a product species (%d) cannot be a reactant", i);
-    PIC_REQUIRE(type == PIC_FUSION_DT_NHE4 || type == PIC_FUSION_DD_PT || type == PIC_FUSION_DD_NHE3,
-                "pic_engine_add_fusion: unknown fusion type %d", type);
     PIC_REQUIRE(multiplier > 0.0 && probability_threshold > 0.0 && probability_target_value > 0.0,
                 "pic_engine_add_fusion: the multiplier, threshold and target value must be positive");
     PIC_REQUIRE(ndt >= 1, "pic_engine_add_fusion: ndt must be at least 1 (got %d)", ndt);
@@ -1388,5 +1420,13 @@ extern "C" int pic_engine_set_species_next_id(void* h, int isp, uint64_t next_id
     PIC_REQUIRE(next_id >= (uint64_t)sp.buf[sp.cur].np, "pic_engine_set_species_next_id: %llu is below the %ld particles",
                 (unsigned long long)next_id, (long)sp.buf[sp.cur].np);
     sp.next_id = next_id;
+    return 0;
+}
+
+extern "C" int pic_engine_set_species_flags(void* h, int isp, int do_not_push, int do_not_deposit) {
+    Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e && isp >= 0 && isp < (int)e->species.size(), "pic_engine_set_species_flags: no species %d", isp);
+    e->species[isp].do_not_push = do_not_push != 0;
+    e->species[isp].do_not_deposit = do_not_deposit != 0;
     return 0;
 }

@@ -1,4 +1,5 @@
-// Two-product nuclear fusion (collisions.collision_names, <name>.type = nuclearfusion) over the rank's box.
+// Nuclear fusion (collisions.collision_names, <name>.type = nuclearfusion) over the rank's box: two-product reactions and
+// proton-boron.
 //
 // Restates, for one tile = the rank's box (paths relative to Source/Particles/Collision/BinaryCollision/):
 //   fuse_cell / chains   <- BinaryCollision::doCollisionsWithinTile  BinaryCollision.H:383-472 (intra-species, halves),
@@ -9,6 +10,9 @@
 //   product_momenta      <- TwoProductFusionComputeProductMomenta + RandomizeVelocity  NuclearFusion/TwoProductFusionUtil.H,
 //                                                                                      Utils/ParticleUtils.H:137-175
 //   create_kernel        <- ParticleCreationFunc::operator() for two products          ParticleCreationFunc.H:120-230
+//   proton_boron         <- ProtonBoronFusionCrossSection (Tentori + Buck)             NuclearFusion/ProtonBoronFusionCrossSection.H
+//   alpha_momenta        <- ProtonBoronFusionInitializeMomentum                        NuclearFusion/ProtonBoronFusionInitializeMomentum.H
+//   create_kernel<true>  <- ParticleCreationFunc::operator() for p + B11 -> 3 alpha    ParticleCreationFunc.H:170-200
 //
 // Determinism: the result is a function of (the particles of each cell by id, seed, collision index, step, global cell)
 // and nothing else -- not of the storage order or the thread mapping.  The Coulomb pass's contract (collision.cu), with:
@@ -19,9 +23,11 @@
 //     1 shuffle species 1 and 2, tag 2 + c is pair chain c and draws ONE uniform per pair that reaches
 //     SingleNuclearFusionEvent (pairs with a spent reactant draw nothing, NuclearFusionFunc.H:181-184).  The momenta of
 //     the products of the cell's j-th event (in pair order) come from the stream with bit 62 also set in the last word:
-//     (2^63 | 2^62 | collision index << 32 | j), two uniforms (RandomizeVelocity's theta, then z);
+//     (2^63 | 2^62 | collision index << 32 | j), two uniforms (RandomizeVelocity's theta, then z); for proton-boron
+//     four (one Philox4x64 block): theta and z of the alpha + 8Be* emission, then theta and z of the 8Be* decay;
 //   * product order: event e of the call counts events bin by bin (the supercell-major order of pic_bins), then by
-//     pair index inside the cell (the chain position k of NuclearFusionFunc.H's pair_index);
+//     pair index inside the cell (the chain position k of NuclearFusionFunc.H's pair_index); a two-product event
+//     writes slots 2e, 2e + 1 of each product, a proton-boron event slots 6e + 2k, 6e + 2k + 1 of alpha k = 0, 1, 2;
 //   * the file is compiled without FMA contraction.
 //
 // Event pass: one pass over the bins with the Coulomb pass's grouping -- a warp per cell of at most SMALL_CAP
@@ -45,6 +51,9 @@ using coll::PI;
 
 constexpr double Q_E = 1.602176634e-19;         // PhysConst::q_e
 constexpr double ALPHA = 0.007297352573748943;  // PhysConst::alpha
+constexpr double M_U = 1.66053906660e-27;      // PhysConst::m_u
+constexpr double EP0 = 8.8541878128e-12;       // PhysConst::ep0
+constexpr double HBAR = 1.054571817e-34;       // PhysConst::hbar
 constexpr double C_SQ = C_LIGHT * C_LIGHT;
 constexpr double INV_CSQ = 1.0 / C_SQ;
 
@@ -158,6 +167,49 @@ __host__ __device__ __forceinline__ double bosch_hale(double E, int type, double
     return millibarn_to_sqm * astrophysical_factor / E_keV * exp(-B_G / sqrt(E_keV));
 }
 
+// ProtonBoronFusionCrossSectionTentori [barn] of the centre-of-momentum kinetic energy in keV (0 < E < 9.76 MeV)
+__host__ __device__ __forceinline__ double pb_tentori(double E_keV) {
+    if (E_keV == 0.0) return 0.0;
+    const double E_MeV = E_keV * 1.e-3;
+    constexpr double joule_to_MeV = 1.e-6 / Q_E;
+    constexpr double one_pr = 1.0;
+    constexpr double Z_boron = 5.0;
+    constexpr double m_boron = 11.00930536 * M_U;
+    constexpr double m_hydrogen = 1.00782503223 * M_U;
+    constexpr double m_reduced = m_boron / (one_pr + m_boron / m_hydrogen);
+    constexpr double gamow_factor = m_reduced / 2.0 * (Q_E * Q_E * Z_boron / (2.0 * EP0 * HBAR)) *
+                                    (Q_E * Q_E * Z_boron / (2.0 * EP0 * HBAR)) * joule_to_MeV;
+    double astrophysical_factor;
+    if (E_keV < 400.0) {
+        constexpr double C0 = 197.0, C1 = 0.269, C2 = 2.54e-4, AL = 1.82e4, EL = 148.0, dEL_sq = 2.35 * 2.35;
+        astrophysical_factor = C0 + C1 * E_keV + C2 * (E_keV * E_keV) + AL / ((E_keV - EL) * (E_keV - EL) + dEL_sq);
+    } else if (E_keV < 668.0) {
+        constexpr double D0 = 346.0, D1 = 150.0, D2 = -59.9, D5 = -0.460;
+        const double E_norm = (E_keV - 400.0) * 1.e-2;
+        const double E_norm_sq = E_norm * E_norm;
+        // amrex::Math::powi<5>(x) = x * powi<2>(powi<2>(x))
+        astrophysical_factor = D0 + D1 * E_norm + D2 * E_norm_sq + D5 * (E_norm * (E_norm_sq * E_norm_sq));
+    } else {
+        constexpr double A0 = 1.98e6, A1 = 3.89e6, A2 = 1.36e6, A3 = 3.71e6;
+        constexpr double E0 = 640.9, E1 = 1211.0, E2 = 2340.0, E3 = 3294.0;
+        constexpr double dE0_sq = 85.5 * 85.5, dE1_sq = 414.0 * 414.0, dE2_sq = 221.0 * 221.0, dE3_sq = 351.0 * 351.0;
+        constexpr double B = 0.381;
+        astrophysical_factor = A0 / ((E_keV - E0) * (E_keV - E0) + dE0_sq) + A1 / ((E_keV - E1) * (E_keV - E1) + dE1_sq) +
+                               A2 / ((E_keV - E2) * (E_keV - E2) + dE2_sq) + A3 / ((E_keV - E3) * (E_keV - E3) + dE3_sq) + B;
+    }
+    return astrophysical_factor / E_MeV * exp(-sqrt(gamow_factor / E_MeV));
+}
+
+// ProtonBoronFusionCrossSection [m^2] of the centre-of-momentum kinetic energy E [J]: Tentori up to 9.76 MeV, Buck's
+// power law above
+__host__ __device__ __forceinline__ double proton_boron(double E) {
+    constexpr double joule_to_keV = 1.e-3 / Q_E;
+    const double E_keV = E * joule_to_keV;
+    const double cross_section_b = E_keV <= 9760.0 ? pb_tentori(E_keV)
+                                                   : 0.01277998 * pow(E_keV / 9760.0, -2.661840717596765);
+    return cross_section_b * 1.e-28;
+}
+
 // SingleNuclearFusionEvent: one uniform; returns the reaction weight w_min / multiplier_eff, or 0 without an event
 __host__ __device__ __forceinline__ bool fusion_event(double u1x, double u1y, double u1z, double u2x, double u2y,
                                                      double u2z, double m1, double m2, double w1, double w2, double dt,
@@ -167,7 +219,7 @@ __host__ __device__ __forceinline__ bool fusion_event(double u1x, double u1y, do
     collision_parameters(u1x, u1y, u1z, u2x, u2y, u2z, m1, m2, E_coll, v_coll, lab_to_com);
     const double w_min = dmin(w1, w2);
     const double w_max = dmax(w1, w2);
-    const double sigma = bosch_hale(E_coll, type, m1, m2);
+    const double sigma = type == PIC_FUSION_PB_3HE4 ? proton_boron(E_coll) : bosch_hale(E_coll, type, m1, m2);
     double pe = multiplier_ratio * mult * lab_to_com * w_max * sigma * v_coll * dt / dV;
     double mult_eff = mult;
     if (pe > thr) {
@@ -229,6 +281,49 @@ __host__ __device__ __forceinline__ void product_momenta(double u1x, double u1y,
 
 __host__ __device__ __forceinline__ double fusion_energy(int type) {   // ParticleCreationFunc.H:205-217
     return type == PIC_FUSION_DT_NHE4 ? 17.5893e6 * Q_E : (type == PIC_FUSION_DD_PT ? 4.032667e6 * Q_E : 3.268911e6 * Q_E);
+}
+
+// ProtonBoronFusionInitializeMomentum: p + B11 -> alpha + 8Be* (isotropic in the centre-of-momentum frame), then
+// 8Be* -> 2 alpha (isotropic in its rest frame, boosted back with Perez eq. 13).  u[k] is alpha k's momentum.
+__host__ __device__ __forceinline__ void alpha_momenta(double u1x, double u1y, double u1z, double m1, double u2x,
+                                                       double u2y, double u2z, double m2, Stream& rng, double u[3][3]) {
+    constexpr double mev_to_joule = Q_E * 1.e6;
+    constexpr double E_fusion = 5.55610759 * mev_to_joule;
+    constexpr double E_decay = 3.12600414 * mev_to_joule;
+    constexpr double m_alpha = M_U * 4.00260325413;
+    constexpr double m_beryllium = M_U * (8.0053095729 + 0.00325283863);
+    constexpr double mBe_sq = m_beryllium * m_beryllium;
+    double uBe[3];
+    product_momenta(u1x, u1y, u1z, m1, u2x, u2y, u2z, m2, m_alpha, m_beryllium, E_fusion, rng, u[0], uBe);
+    const double px_Be = m_beryllium * uBe[0], py_Be = m_beryllium * uBe[1], pz_Be = m_beryllium * uBe[2];
+    constexpr double gamma_Bestar = 1.0 + 0.5 * E_decay / (m_alpha * C_SQ);
+    constexpr double gamma_Bestar_sq_minus_one = gamma_Bestar * gamma_Bestar - 1.0;
+    const double p_Bestar = m_alpha * C_LIGHT * sqrt(gamma_Bestar_sq_minus_one);
+    // RandomizeVelocity(px*, py*, pz*, p_Bestar): theta, then z
+    const double theta = rng.uniform() * 2.0 * PI;
+    const double z = 2.0 * rng.uniform() - 1.0;
+    const double xy = sqrt(1.0 - z * z);
+    double st, ct;
+#ifdef __CUDA_ARCH__
+    sincos(theta, &st, &ct);
+#else
+    st = sin(theta); ct = cos(theta);
+#endif
+    const double px_s = xy * ct * p_Bestar, py_s = xy * st * p_Bestar, pz_s = z * p_Bestar;
+    const double p_Be_sq = px_Be * px_Be + py_Be * py_Be + pz_Be * pz_Be;
+    const double g_Be = sqrt(1.0 + p_Be_sq / (mBe_sq * C_SQ));
+    const double mg_Be = m_beryllium * g_Be;
+    const double vx = px_Be / mg_Be, vy = py_Be / mg_Be, vz = pz_Be / mg_Be;
+    const double v_Be_sq = vx * vx + vy * vy + vz * vz;
+    double px2 = px_s, py2 = py_s, pz2 = pz_s;
+    if (v_Be_sq > DBL_MIN_) {
+        const double vcDps = vx * px_s + vy * py_s + vz * pz_s;
+        const double factor0 = (g_Be - 1.0) / v_Be_sq;
+        const double factor = factor0 * vcDps + m_alpha * gamma_Bestar * g_Be;
+        px2 = px_s + vx * factor; py2 = py_s + vy * factor; pz2 = pz_s + vz * factor;
+    }
+    u[1][0] = px2 / m_alpha; u[1][1] = py2 / m_alpha; u[1][2] = pz2 / m_alpha;
+    u[2][0] = (px_Be - px2) / m_alpha; u[2][1] = (py_Be - py2) / m_alpha; u[2][2] = (pz_Be - pz2) / m_alpha;
 }
 
 // first record slot of the bin's pairs: [cs1 + cs2, + n1 + n2) of one bin never overlaps another's
@@ -501,7 +596,9 @@ struct CreateArgs {
     Work wk;
 };
 
-// a warp per bin: the bin's events in pair order, event e of the call at offsets[bin] + (its rank in the bin)
+// a warp per bin: the bin's events in pair order, event e of the call at offsets[bin] + (its rank in the bin).  PB: the
+// proton-boron reaction, six alphas per event in product A.
+template <bool PB>
 __global__ void __launch_bounds__(128) create_kernel(CreateArgs a, long nbins) {
     const int lane = threadIdx.x & 31;
     const long stride = (long)gridDim.x * 4;
@@ -523,23 +620,38 @@ __global__ void __launch_bounds__(128) create_kernel(CreateArgs a, long nbins) {
                 const SoaView& Q = a.same ? a.P1 : a.P2;
                 const double m2 = a.same ? a.m1 : a.m2;
                 Stream rng(a.seed, a.step, gcell, PRODUCT_TAG | (a.cidx << 32) | (uint64_t)j);
-                double uA[3], uB[3];
-                product_momenta(a.P1.ux[p1], a.P1.uy[p1], a.P1.uz[p1], a.m1, Q.ux[p2], Q.uy[p2], Q.uz[p2], m2, a.mA,
-                                a.mB, E_fusion, rng, uA, uB);
                 const double wh = a.wk.wr[base + k] / 2.0;
-                for (int prod = 0; prod < 2; ++prod) {
-                    const SoaView& P = prod ? a.PB : a.PA;
-                    uint64_t* id = prod ? a.idB : a.idA;
-                    const double* u = prod ? uB : uA;
-                    const uint64_t first = prod ? a.next_idB : a.next_idA;
-                    for (int side = 0; side < 2; ++side) {
-                        const long o = 2 * e + side;                       // P's pointers start at its old np
-                        const SoaView& S = side ? Q : a.P1;
-                        const int p = side ? p2 : p1;
-                        P.x[o] = S.x[p]; P.y[o] = S.y[p]; P.z[o] = S.z[p];
-                        P.ux[o] = u[0]; P.uy[o] = u[1]; P.uz[o] = u[2];
-                        P.w[o] = wh;
-                        id[o] = first + (uint64_t)o;
+                if constexpr (PB) {
+                    double u[3][3];
+                    alpha_momenta(a.P1.ux[p1], a.P1.uy[p1], a.P1.uz[p1], a.m1, Q.ux[p2], Q.uy[p2], Q.uz[p2], m2, rng, u);
+                    for (int al = 0; al < 3; ++al)
+                        for (int side = 0; side < 2; ++side) {
+                            const long o = 6 * e + 2 * al + side;          // PA's pointers start at its old np
+                            const SoaView& S = side ? Q : a.P1;
+                            const int p = side ? p2 : p1;
+                            a.PA.x[o] = S.x[p]; a.PA.y[o] = S.y[p]; a.PA.z[o] = S.z[p];
+                            a.PA.ux[o] = u[al][0]; a.PA.uy[o] = u[al][1]; a.PA.uz[o] = u[al][2];
+                            a.PA.w[o] = wh;
+                            a.idA[o] = a.next_idA + (uint64_t)o;
+                        }
+                } else {
+                    double uA[3], uB[3];
+                    product_momenta(a.P1.ux[p1], a.P1.uy[p1], a.P1.uz[p1], a.m1, Q.ux[p2], Q.uy[p2], Q.uz[p2], m2, a.mA,
+                                    a.mB, E_fusion, rng, uA, uB);
+                    for (int prod = 0; prod < 2; ++prod) {
+                        const SoaView& P = prod ? a.PB : a.PA;
+                        uint64_t* id = prod ? a.idB : a.idA;
+                        const double* u = prod ? uB : uA;
+                        const uint64_t first = prod ? a.next_idB : a.next_idA;
+                        for (int side = 0; side < 2; ++side) {
+                            const long o = 2 * e + side;                       // P's pointers start at its old np
+                            const SoaView& S = side ? Q : a.P1;
+                            const int p = side ? p2 : p1;
+                            P.x[o] = S.x[p]; P.y[o] = S.y[p]; P.z[o] = S.z[p];
+                            P.ux[o] = u[0]; P.uy[o] = u[1]; P.uz[o] = u[2];
+                            P.w[o] = wh;
+                            id[o] = first + (uint64_t)o;
+                        }
                     }
                 }
             }
@@ -572,10 +684,10 @@ static int check_fusion(const char* what, const pic_fusion_collision* c, const p
     PIC_REQUIRE(c && p1 && b1, "%s: null argument", what);
     PIC_REQUIRE(b1->cell_start && b1->np_binned == p1->np, "%s: species 1 needs current bins", what);
     PIC_REQUIRE(p1->idcpu && p1->w, "%s: species 1 needs ids and weights", what);
-    PIC_REQUIRE(c->type == PIC_FUSION_DT_NHE4 || c->type == PIC_FUSION_DD_PT || c->type == PIC_FUSION_DD_NHE3,
-                "%s: unknown fusion type %d", what, c->type);
-    PIC_REQUIRE(c->m1 > 0.0 && (c->same_species || c->m2 > 0.0) && c->mA > 0.0 && c->mB > 0.0,
-                "%s: masses must be positive", what);
+    PIC_REQUIRE(c->type == PIC_FUSION_DT_NHE4 || c->type == PIC_FUSION_DD_PT || c->type == PIC_FUSION_DD_NHE3 ||
+                c->type == PIC_FUSION_PB_3HE4, "%s: unknown fusion type %d", what, c->type);
+    PIC_REQUIRE(c->m1 > 0.0 && (c->same_species || c->m2 > 0.0) && c->mA > 0.0 &&
+                (c->type == PIC_FUSION_PB_3HE4 || c->mB > 0.0), "%s: masses must be positive", what);
     PIC_REQUIRE(c->fusion_multiplier > 0.0, "%s: the fusion multiplier must be positive", what);
     if (!c->same_species) {
         PIC_REQUIRE(p2 && b2 && b2->cell_start && b2->np_binned == p2->np && p2->idcpu && p2->w,
@@ -640,8 +752,10 @@ extern "C" int pic_fusion_create_products(const pic_fusion_collision* c, const p
                                           uint64_t next_idA, const pic_soa* pB, long capB, uint64_t next_idB,
                                           long* n_events, void* stream) {
     if (int rc = check_fusion("pic_fusion_create_products", c, p1, b1, p2, b2)) return rc;
-    PIC_REQUIRE(g && work && pA && pB && n_events, "pic_fusion_create_products: null argument");
-    PIC_REQUIRE(pA->idcpu && pA->w && pB->idcpu && pB->w, "pic_fusion_create_products: products need ids and weights");
+    const bool pb = c->type == PIC_FUSION_PB_3HE4;
+    PIC_REQUIRE(g && work && pA && (pb || pB) && n_events, "pic_fusion_create_products: null argument");
+    PIC_REQUIRE(pA->idcpu && pA->w && (pb || (pB->idcpu && pB->w)),
+                "pic_fusion_create_products: products need ids and weights");
     *n_events = 0;
     fus::CreateArgs a;
     a.b1 = make_bins(*b1);
@@ -655,23 +769,27 @@ extern "C" int pic_fusion_create_products(const pic_fusion_collision* c, const p
     cudaMemcpyAsync(&total, a.wk.offsets + nbins, sizeof(int), cudaMemcpyDeviceToHost, s);
     if (cudaStreamSynchronize(s) != cudaSuccess)
         return fail("pic_fusion_create_products: %s", cudaGetErrorString(cudaGetLastError()));
-    PIC_REQUIRE(pA->np + 2L * total <= capA, "pic_fusion_create_products: product A needs a capacity of %ld (has %ld)",
-                pA->np + 2L * total, capA);
-    PIC_REQUIRE(pB->np + 2L * total <= capB, "pic_fusion_create_products: product B needs a capacity of %ld (has %ld)",
-                pB->np + 2L * total, capB);
+    const long per_event = pb ? 6L : 2L;
+    PIC_REQUIRE(pA->np + per_event * total <= capA,
+                "pic_fusion_create_products: product A needs a capacity of %ld (has %ld)", pA->np + per_event * total, capA);
+    PIC_REQUIRE(pb || pB->np + 2L * total <= capB,
+                "pic_fusion_create_products: product B needs a capacity of %ld (has %ld)", pB->np + 2L * total, capB);
     *n_events = total;
     if (total == 0) return 0;
     a.P1 = make_soa(*p1, 0);
     a.P2 = c->same_species ? a.P1 : make_soa(*p2, 0);
-    a.PA = make_soa(*pA, pA->np); a.PB = make_soa(*pB, pB->np);
-    a.idA = pA->idcpu + pA->np; a.idB = pB->idcpu + pB->np;
+    a.PA = make_soa(*pA, pA->np);
+    a.idA = pA->idcpu + pA->np;
+    if (!pb) { a.PB = make_soa(*pB, pB->np); a.idB = pB->idcpu + pB->np; }
     a.gn[0] = g->n_cell[0]; a.gn[1] = g->n_cell[1];
     a.same = c->same_species; a.type = c->type;
     a.m1 = c->m1; a.m2 = c->m2; a.mA = c->mA; a.mB = c->mB;
     a.seed = c->seed; a.cidx = (uint64_t)(uint32_t)c->collision_index; a.step = (uint64_t)step;
     a.next_idA = next_idA; a.next_idB = next_idB;
     const long blocks = (nbins + 3) / 4;
-    fus::create_kernel<<<(unsigned)(blocks < 2147483647L ? blocks : 2147483647L), 128, 0, s>>>(a, nbins);
+    const unsigned grid = (unsigned)(blocks < 2147483647L ? blocks : 2147483647L);
+    if (pb) fus::create_kernel<true><<<grid, 128, 0, s>>>(a, nbins);
+    else fus::create_kernel<false><<<grid, 128, 0, s>>>(a, nbins);
     count_launch();
     return check_launch("pic_fusion_create_products") ? 0 : 1;
 }

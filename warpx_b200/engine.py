@@ -164,6 +164,7 @@ class Species:
             self.buf[0][n, :self.np].copy_(src, non_blocking=True)
         self.cell_start = None    # cell-sort scratch of the C++ driver (Simulation._register_species), none without bins
         self.work = None
+        self.do_not_push = self.do_not_deposit = False     # Simulation.set_species_flags
 
     def soa(self, which=None):
         b = self.buf[self.cur if which is None else which]
@@ -192,6 +193,7 @@ SPECIES_PROPERTIES = {
     "hydrogen3": (1 * Q_E, 3.0160492779 * M_U),
     "helium3": (2 * Q_E, 3.0160293201 * M_U),
     "helium4": (2 * Q_E, 4.00260325413 * M_U),
+    "boron11": (5 * Q_E, 11.00930536 * M_U),
 }
 
 
@@ -209,9 +211,13 @@ def species_charge_mass(species_type):
 
 
 def nuclear_fusion_type(reactants, products):
-    """BinaryCollisionUtils::get_nuclear_fusion_type (BinaryCollisionUtils.cpp:40-123) for the two-product reactions:
-    the abi.FUSION_* of the reactants' and products' species types; other combinations are refused."""
+    """BinaryCollisionUtils::get_nuclear_fusion_type (BinaryCollisionUtils.cpp:40-123) for the two-product reactions
+    and proton-boron: the abi.FUSION_* of the reactants' and products' species types; other combinations are refused."""
     r, p = sorted(reactants), sorted(products)
+    if r == ["boron11", "hydrogen1"]:                  # :104-116
+        if p != ["helium4"]:
+            raise ValueError("proton-boron fusion: exactly one product species, of type helium4")
+        return abi.FUSION_PB_3HE4
     if r == ["hydrogen2", "hydrogen3"]:
         if p != ["helium4", "neutron"]:
             raise ValueError("deuterium-tritium fusion: the products must be of type neutron and helium4")
@@ -223,8 +229,8 @@ def nuclear_fusion_type(reactants, products):
             return abi.FUSION_DD_PT
         raise ValueError("deuterium-deuterium fusion: the products must be of type helium3 and neutron, or hydrogen3 and "
                          "hydrogen1")
-    raise NotImplementedError("nuclear fusion between species of type %s and %s is not supported (D + T and D + D only)"
-                              % tuple(reactants))
+    raise NotImplementedError("nuclear fusion between species of type %s and %s is not supported (D + T, D + D and "
+                              "p + B11 only)" % tuple(reactants))
 
 
 class FluidSpecies:
@@ -547,20 +553,22 @@ class Simulation:
                    probability_target_value=0.002, ndt=1, seed=0):
         """One entry of collisions.collision_names with <name>.type = nuclearfusion: <name>.species = species1 species2
         (the same species twice: D + D within one species), <name>.product_species = products (two species, in the
-        order the products are written), <name>.fusion_multiplier, fusion_probability_threshold,
-        fusion_probability_target_value and ndt.  The reaction follows from the species types, as
-        get_nuclear_fusion_type infers it: D + T -> n + He4, D + D -> n + He3 or p + T.  Products appear at their
+        order the products are written; one helium4 species for proton-boron), <name>.fusion_multiplier,
+        fusion_probability_threshold, fusion_probability_target_value and ndt.  The reaction follows from the species
+        types, as get_nuclear_fusion_type infers it: D + T -> n + He4, D + D -> n + He3 or p + T, p + B11 -> 3 He4 (six
+        alphas of weight w / 2 per event, three at each reactant's position).  Products appear at their
         reactants' positions; reactants whose weight is used up leave the run at the end of the step.  It shares the
         collision index, the schedule and the determinism of add_collision.  One rank only.  Returns the index."""
         isp = [self._species_index(v) for v in (species1, species2)]
-        if len(products) != 2:
-            raise ValueError("add_fusion: a two-product fusion takes exactly two product species")
+        if len(products) not in (1, 2):
+            raise ValueError("add_fusion: a fusion takes one or two product species")
         ipr = [self._species_index(v) for v in products]
         types = [self.species[i].species_type for i in isp + ipr]
         if any(v is None for v in types):
             raise ValueError("add_fusion: every reactant and product needs a species_type")
         ftype = nuclear_fusion_type(types[:2], types[2:])
-        check(self.L.pic_engine_add_fusion(self.native, isp[0], isp[1], ipr[0], ipr[1], ftype, float(multiplier),
+        ipr_b = ipr[1] if len(ipr) == 2 else -1
+        check(self.L.pic_engine_add_fusion(self.native, isp[0], isp[1], ipr[0], ipr_b, ftype, float(multiplier),
                                            float(probability_threshold), float(probability_target_value), int(ndt),
                                            int(seed)))
         self.collisions.append(dict(species=tuple(isp), products=tuple(ipr), type=ftype, multiplier=float(multiplier),
@@ -568,6 +576,16 @@ class Simulation:
                                     probability_target_value=float(probability_target_value), ndt=int(ndt),
                                     seed=int(seed)))
         return len(self.collisions) - 1
+
+    def set_species_flags(self, species, do_not_push=False, do_not_deposit=False):
+        """<species>.do_not_push / <species>.do_not_deposit of a species (a Species object, name or index), also one that
+        read_checkpoint restored (checkpoints do not carry the flags).  do_not_push: the species' positions and momenta
+        keep their bits while it is still sorted, collided, fused and wrapped; do_not_deposit: it is pushed but adds
+        nothing to J or to rho_numpy().  Immobile targets, test species and diagnostics-only species use them."""
+        isp = self._species_index(species)
+        check(self.L.pic_engine_set_species_flags(self.native, isp, 1 if do_not_push else 0, 1 if do_not_deposit else 0))
+        sp = self.species[isp]
+        sp.do_not_push, sp.do_not_deposit = bool(do_not_push), bool(do_not_deposit)
 
     def species_next_id(self, isp):
         """The id the next particle species isp creates receives (its id counter)."""
@@ -691,7 +709,7 @@ class Simulation:
 
     def rho_numpy(self):
         """The `rho` diagnostic of a plotfile (Diagnostics/ComputeDiagFunctors/RhoFunctor.cpp:35-81): every
-        container (species, then laser antennas) deposits its charge on a nodal array with ng_depos_rho guard
+        container (species without do_not_deposit, then laser antennas) deposits its charge on a nodal array with ng_depos_rho guard
         cells and applies the PEC / reflecting image charge, the containers are added, then
         WarpX::ApplyFilterandSumBoundaryRho (Parallelization/WarpXComm.cpp:1552-1568).  Returns
         (descriptor, numpy array [k, j, i]).  One rank."""
@@ -710,7 +728,7 @@ class Simulation:
         rho_d, rho = make((ng,) * 3)
         one_d, one = make((ng,) * 3)
         xyzmin, lo = self.lower_corner((ng,) * 3)
-        containers = [(sp.soa(), sp.q) for sp in self.species]
+        containers = [(sp.soa(), sp.q) for sp in self.species if not sp.do_not_deposit]   # MultiParticleContainer.cpp:576,598
         for il, la in enumerate(self.lasers):
             soa = abi.pic_soa()
             for k, name in enumerate(Species.NAMES):

@@ -390,3 +390,178 @@ def particle_boundaries_3d():
                 field_lo=("pec", "pec", "periodic"), field_hi=("pec", "pec", "periodic"),
                 particle_lo=("reflecting", "absorbing", "periodic"), particle_hi=("reflecting", "absorbing", "periodic"),
                 nox=1, use_filter=True, cfl=1.0, max_step=8, species=species)
+
+
+# ---- the reference's 3D nuclear fusion decks (Examples/Tests/nuclear_fusion/inputs_test_3d_*) ----------------------
+M_U = 1.66053906660e-27
+_FUSION_MASS = {"hydrogen1": 1.00782503223 * M_U, "hydrogen2": 2.01410177812 * M_U, "hydrogen3": 3.0160492779 * M_U,
+                "helium3": 3.0160293201 * M_U, "helium4": 4.00260325413 * M_U, "boron11": 11.00930536 * M_U,
+                "neutron": 1.0013784193052508 * 1.67262192369e-27}
+_FUSION_CHARGE = {"hydrogen1": 1, "hydrogen2": 1, "hydrogen3": 1, "helium3": 2, "helium4": 2, "boron11": 5, "neutron": 0}
+
+
+def _fusion_species(name, species_type, seed, geom, ppc, density, u):
+    """NRandomPerCell species of a fusion deck, not pushed and not depositing: density(x, y, z) [m^-3] and u(x, y, z) ->
+    (ux, uy, uz) in units of c, evaluated at the particles' positions; w = density dV / ppc."""
+    x, y, z = _random_per_cell(seed, geom[0], geom[1], geom[2], ppc)
+    dV = np.prod((np.asarray(geom[2]) - np.asarray(geom[1])) / np.asarray(geom[0]))
+    ux, uy, uz = (np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), x.shape) * C) for v in u(x, y, z))
+    w = np.ascontiguousarray(np.broadcast_to(np.asarray(density(x, y, z), dtype=np.float64), x.shape) * dV / ppc)
+    return dict(name=name, species_type=species_type, q=_FUSION_CHARGE[species_type] * Q_E, m=_FUSION_MASS[species_type],
+                x=x, y=y, z=z, w=w, ux=ux, uy=uy, uz=uz, do_not_push=True, do_not_deposit=True)
+
+
+def _merge(name, a, b):
+    """<species>.injection_sources: the particles of two sources in one species"""
+    out = dict(a, name=name)
+    for k in ("x", "y", "z", "w", "ux", "uy", "uz"):
+        out[k] = np.concatenate([a[k], b[k]])
+    return out
+
+
+def _product(name, species_type, capacity):
+    return dict(name=name, species_type=species_type, capacity=int(capacity), do_not_push=True, do_not_deposit=True)
+
+
+def _thermal(seed, theta):
+    """maxwell_boltzmann with theta (InjectorMomentumBoltzmann, no drift): per component N(0, sqrt(theta)) in units of c"""
+    def u(x, y, z):
+        g = philox_normal(seed, 0, len(x))
+        return tuple(np.sqrt(theta) * g[:, d] for d in range(3))
+    return u
+
+
+def _two_product_deck(reaction, scale, seed):
+    """inputs_test_3d_deuterium_tritium_fusion ("dt") and inputs_test_3d_deuterium_deuterium_fusion ("dd")"""
+    geom = ((8, 8, 16), (0.0, 0.0, 0.0), (8.0, 8.0, 16.0))
+    ncell = 8 * 8 * 16
+    keV = 1.e3 * Q_E
+    E_step = 22. * keV
+    m_d, m_t = _FUSION_MASS["hydrogen2"], _FUSION_MASS["hydrogen3"]
+    n1 = max(int(10000 * scale), 2)
+    if reaction == "dt":
+        m_r = m_d * m_t / (m_d + m_t)
+        r2, m2 = "hydrogen3", m_t
+        uz1 = lambda x, y, z: (0.0, 0.0, np.sqrt(2 * m_r * E_step * np.floor(z) ** 2) / (m_d * C))
+        uz2 = lambda x, y, z: (0.0, 0.0, -np.sqrt(2 * m_r * E_step * np.floor(z) ** 2) / (m_t * C))
+        prods = ("helium4", "neutron")
+    else:
+        r2, m2 = "hydrogen2", m_d
+        uz1 = lambda x, y, z: (0.0, 0.0, np.sqrt(m_d * E_step * np.floor(z) ** 2) / (m_d * C))
+        uz2 = lambda x, y, z: (0.0, 0.0, -np.sqrt(m_d * E_step * np.floor(z) ** 2) / (m_d * C))
+        prods = ("helium3", "neutron")
+    one = lambda x, y, z: 1.0
+    species = [_fusion_species("reactant1_1", "hydrogen2", seed, geom, n1, one, uz1),
+               _fusion_species("reactant2_1", r2, seed + 2, geom, n1, one, uz2),
+               _product("product1_1", prods[0], 2 * n1 * ncell), _product("product2_1", prods[1], 2 * n1 * ncell)]
+    fusions = [dict(species=(0, 1), products=(2, 3), multiplier=1e50, threshold=0.02, target=0.002)]
+    sets = [dict(reactants=(0, 1), products=(2, 3), pairs_per_cell=n1, densities=(1.0, 1.0), target=0.002)]
+    if reaction == "dt":
+        bg, beam = 1.e26, 1.e20
+        nh, nl, n2 = max(int(100 * scale), 1), max(int(900 * scale), 1), max(int(100 * scale), 1)
+        high = _fusion_species("d2", "hydrogen2", seed + 4, geom, nh, lambda x, y, z: 10. * bg, lambda x, y, z: (0., 0., 0.))
+        low = _fusion_species("d2", "hydrogen2", seed + 6, geom, nl, lambda x, y, z: 10. / 9. * beam,
+                              lambda x, y, z: (0.0, 0.0, np.sqrt(2 * m_d * E_step * np.floor(z) ** 2) / (m_d * C)))
+        species += [_merge("reactant1_2", high, low),
+                    _fusion_species("reactant2_2", "hydrogen3", seed + 8, geom, n2, lambda x, y, z: bg,
+                                    lambda x, y, z: (0., 0., 0.)),
+                    _product("product1_2", "helium4", 2 * (nh + nl) * ncell),
+                    _product("product2_2", "neutron", 2 * (nh + nl) * ncell)]
+        fusions.append(dict(species=(4, 5), products=(6, 7), multiplier=1e15, threshold=0.02, target=0.02))
+        # each injection source weighs its own particles: the beam is 900 particles per cell at 10/9 beam_dens
+        sets.append(dict(reactants=(4, 5), products=(6, 7), pairs_per_cell=nl, densities=(10. / 9. * beam, bg),
+                         target=0.02, beam_only=True))
+    return dict(n_cell=geom[0], prob_lo=geom[1], prob_hi=geom[2], nox=1, cfl=1.0, max_step=1, seed=seed,
+                species=species, fusions=fusions,
+                analysis=dict(reaction=reaction, E_step=E_step, sets=sets, tol=1e-12, energy_tol=1e-8,
+                              isotropy=0.03, xy_isotropy=0.05, rho_tol=2e-11))
+
+
+def fusion_dt_3d(scale=1.0, seed=4):
+    """Examples/Tests/nuclear_fusion/inputs_test_3d_deuterium_tritium_fusion: 8 x 8 x 16 cells of 1 m, order 1, Yee with
+    cfl 1, one step; every species is not pushed and does not deposit.  Set 1: 10 000 D + 10 000 T per cell at momenta
+    constant per z slice (E* = 22 keV floor(z)^2), fusion_multiplier 1e50.  Set 2: D of two injection sources (100 at
+    rest at 1e27 m^-3 and 900 of a beam at 1.1e20 m^-3 per cell) on 100 T at rest at 1e26 m^-3, multiplier 1e15, target
+    value 0.02.  scale multiplies the particles per cell (1 is the deck)."""
+    return _two_product_deck("dt", scale, seed)
+
+
+def fusion_dd_3d(scale=1.0, seed=5):
+    """Examples/Tests/nuclear_fusion/inputs_test_3d_deuterium_deuterium_fusion: set 1 of the D-T deck with two deuterium
+    species in head-on beams (E* = 22 keV floor(z)^2) fusing into He3 + n."""
+    return _two_product_deck("dd", scale, seed)
+
+
+def fusion_dd_intraspecies_3d(scale=1.0, seed=1034958209):
+    """Examples/Tests/nuclear_fusion/inputs_test_3d_deuterium_deuterium_fusion_intraspecies: 8^3 cells over
+    [-1 mm, 1 mm]^3, Yee with cfl 1, 10 steps; 10 000 deuterons per cell at 1e26 m^-3 with a gaussian thermal
+    spread of 0.003265007901313691 c per component, D + D -> He3 + n within the species with multiplier 1e10.  The
+    analysis reads <sigma v> from the neutrons' ParticleNumber history: 2.603e-18 cm^3/s within 2 %."""
+    geom = ((8, 8, 8), (-1e-3,) * 3, (1e-3,) * 3)
+    n = max(int(10000 * scale), 2)
+    u_th = 0.003265007901313691
+    def u(x, y, z):
+        g = philox_normal(seed + 1, 0, len(x))
+        return tuple(u_th * g[:, d] for d in range(3))
+    d = _fusion_species("deuterium", "hydrogen2", seed, geom, n, lambda x, y, z: 1e26, u)
+    species = [d, _product("helium3", "helium3", 2 * len(d["x"])), _product("neutron", "neutron", 2 * len(d["x"]))]
+    # The deck uses shape order 3; no species is pushed or deposits, so the order does not enter the result, and 8 cells
+    # per axis are too few for the guard cells of order 3 in this engine's periodic exchange: order 1.
+    return dict(n_cell=geom[0], prob_lo=geom[1], prob_hi=geom[2], nox=1, cfl=1.0, max_step=10, seed=seed,
+                species=species, fusions=[dict(species=(0, 0), products=(1, 2), multiplier=1e10, threshold=0.02,
+                                               target=0.002)],
+                analysis=dict(density=1e26, volume=(2e-3) ** 3, sigma_v=2.603e-18, tolerance=0.02))
+
+
+def proton_boron_3d(scale=1.0, seed=6):
+    """Examples/Tests/nuclear_fusion/inputs_test_3d_proton_boron_fusion: 8 x 8 x 16 cells of 1 m, order 1, Yee with cfl
+    1, one step, five p + B11 -> 3 alpha sets, every species not pushed and not depositing:
+      1. 10 000 p + 10 000 B per cell in head-on beams (E* = 22 keV floor(z)^2), multiplier 1e50;
+      2. 1000 p per cell (a tenth, where y - floor(y) < 0.1, at rest at 1e27 m^-3, the rest a beam at 1.1e20 m^-3 with
+         E = 22 keV floor(z)^2) on 100 B at rest at 1e26 m^-3, multiplier 1e15, target value 0.02;
+      3. 600 p at 1e28 and 1000 B at 5e28 m^-3, Maxwellian at 44 keV, multiplier 1e15;
+      4. 100 p at 1e35 m^-3 with 550 keV on 100 B at rest at 1 m^-3, multiplier 1e21: every boron is used up;
+      5. set 4 with fusion_probability_threshold 1e123: borons remain.
+    scale multiplies the particles per cell (1 is the deck: about 24 M particles)."""
+    geom = ((8, 8, 16), (0.0, 0.0, 0.0), (8.0, 8.0, 16.0))
+    ncell = 8 * 8 * 16
+    keV = 1.e3 * Q_E
+    E_step = 22. * keV
+    m_h, m_b = _FUSION_MASS["hydrogen1"], _FUSION_MASS["boron11"]
+    m_r = m_h * m_b / (m_h + m_b)
+    s = lambda n: max(int(n * scale), 1)
+    at_rest = lambda x, y, z: (0., 0., 0.)
+    bg, beam, T = 1.e26, 1.e20, 44. * keV
+    E4 = 550 * keV
+    p4 = lambda x, y, z: (0., 0., np.sqrt(2 * m_h * E4) / (m_h * C))
+    specs = [
+        (("proton1", "hydrogen1", s(10000), lambda x, y, z: 1.0,
+          lambda x, y, z: (0., 0., np.sqrt(2 * m_r * E_step * np.floor(z) ** 2) / (m_h * C))),
+         ("boron1", "boron11", s(10000), lambda x, y, z: 1.0,
+          lambda x, y, z: (0., 0., -np.sqrt(2 * m_r * E_step * np.floor(z) ** 2) / (m_b * C))), 1e50, 0.02, 0.002),
+        (("proton2", "hydrogen1", s(1000), lambda x, y, z: np.where(y - np.floor(y) < 0.1, 10. * bg, 10. / 9. * beam),
+          lambda x, y, z: (0., 0., np.where(y - np.floor(y) < 0.1, 0.,
+                                            np.sqrt(2 * m_h * E_step * np.floor(z) ** 2) / (m_h * C)))),
+         ("boron2", "boron11", s(100), lambda x, y, z: bg, at_rest), 1e15, 0.02, 0.02),
+        (("proton3", "hydrogen1", s(600), lambda x, y, z: 1e28, _thermal(seed + 101, T / (m_h * C * C))),
+         ("boron3", "boron11", s(1000), lambda x, y, z: 5e28, _thermal(seed + 103, T / (m_b * C * C))), 1e15, 0.02, 0.002),
+        (("proton4", "hydrogen1", s(100), lambda x, y, z: 1e35, p4), ("boron4", "boron11", s(100), lambda x, y, z: 1.0,
+                                                                      at_rest), 1e21, 0.02, 0.002),
+        (("proton5", "hydrogen1", s(100), lambda x, y, z: 1e35, p4), ("boron5", "boron11", s(100), lambda x, y, z: 1.0,
+                                                                      at_rest), 1e21, 1e123, 0.002),
+    ]
+    species, fusions, sets = [], [], []
+    for k, (p, b, mult, thr, target) in enumerate(specs):
+        i = len(species)
+        species.append(_fusion_species(p[0], p[1], seed + 10 * k, geom, p[2], p[3], p[4]))
+        species.append(_fusion_species(b[0], b[1], seed + 10 * k + 2, geom, b[2], b[3], b[4]))
+        species.append(_product("alpha%d" % (k + 1), "helium4", 6 * max(p[2], b[2]) * ncell))
+        fusions.append(dict(species=(i, i + 1), products=(i + 2,), multiplier=mult, threshold=thr, target=target))
+        sets.append(dict(reactants=(i, i + 1), products=(i + 2,), pairs_per_cell=max(p[2], b[2]), target=target))
+    sets[0]["densities"] = (1.0, 1.0)
+    sets[1].update(densities=(beam, bg), pairs_per_cell=int(round(0.9 * s(1000))), beam_only=True)
+    return dict(n_cell=geom[0], prob_lo=geom[1], prob_hi=geom[2], nox=1, cfl=1.0, max_step=1, seed=seed,
+                species=species, fusions=fusions,
+                analysis=dict(reaction="pb", E_step=E_step, sets=sets, tol=1e-12, energy_tol=1e-8, isotropy=0.03,
+                              thermal_isotropy=0.1, xy_isotropy=0.05, thermal=dict(T_keV=44.0, n_p=1e28, n_b=5e28,
+                                                                                    tolerance=0.2), rho_tol=2e-11))
