@@ -12,8 +12,8 @@
 //   handle_particles_at_boundaries <- WarpX::HandleParticlesAtBoundaries   :533-581
 //   guard cells                  <- guardCellManager::Init                 Parallelization/GuardCellManager.cpp:62-161,310-343
 //   dt                           <- WarpX::ComputeDt                       Evolve/WarpXComputeDt.cpp:56-95
-// All memory is borrowed from the caller (fields, particle SoA double buffers, bins, sort scratch);
-// every stage is an asynchronous launch on the caller's stream.
+// Fields, particle SoA double buffers, bins and sort scratch are borrowed from the caller; the driver's own scratch
+// is held in Owned buffers.  Every stage is an asynchronous launch on the caller's stream.
 // Non-periodic domains (pic_engine_set_boundaries / set_moving_window / set_injector / add_laser, one
 // rank): PEC walls after every field push and on J (BoundaryConditions/WarpXFieldBoundaries.cpp:51-190),
 // WarpX::MoveWindow with continuous injection (Utils/WarpXMovingWindow.cpp:139-476), laser antennas
@@ -32,41 +32,107 @@
 
 namespace pic {
 
-extern int g_gather_mode;      // gather_push_tile.cu
+bool gather_push_carries_permutation(int nox);      // gather_push.cu
+
+// Memory the engine owns: device memory, or pinned host memory when Pinned.  The only code in this file that
+// allocates or frees; the memory goes with its owner.  Empty (null) until an allocation succeeds.
+template <class T, bool Pinned = false>
+class Owned {
+public:
+    Owned() = default;
+    Owned(Owned&& o) noexcept { swap(o); }
+    Owned& operator=(Owned&& o) noexcept { Owned(std::move(o)).swap(*this); return *this; }
+    ~Owned() { release(); }
+    // Replaces the memory with `bytes` new bytes.  A failure leaves the buffer empty and clears the sticky error.
+    bool try_alloc(size_t bytes) {
+        release();
+        if ((Pinned ? cudaMallocHost(&p_, bytes) : cudaMalloc(&p_, bytes)) == cudaSuccess) { bytes_ = bytes; return true; }
+        cudaGetLastError();
+        p_ = nullptr;
+        return false;
+    }
+    int alloc(size_t bytes, const char* what) { return try_alloc(bytes) ? 0 : fail("%s", what); }
+    void release() {
+        if (p_) (void)(Pinned ? cudaFreeHost(p_) : cudaFree(p_));
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+    T* get() const { return p_; }
+    size_t bytes() const { return bytes_; }
+    explicit operator bool() const { return p_ != nullptr; }
+private:
+    void swap(Owned& o) noexcept { std::swap(p_, o.p_); std::swap(bytes_, o.bytes_); }
+    T* p_ = nullptr;
+    size_t bytes_ = 0;
+};
+template <class T> using DeviceBuf = Owned<T, false>;
+template <class T> using PinnedBuf = Owned<T, true>;
+
+// How the particles in buf[cur] of a species relate to its cell bins and to its escape list, changed only by the
+// transitions below, which are named after what happened to the particles.
+// A sort inside pic_engine_evolve stops at the permutation: the bins describe the new order, the particles still lie
+// in buf[cur] in the old one, and the next gather + push moves them while it reads them anyway.  Everything else that
+// reads particle arrays carries out the pending move first; no exported call returns with a permutation pending.
+class ParticleOrder {
+public:
+    explicit ParticleOrder(const pic_bins& geometry) : bins_(geometry) { bins_.np_binned = 0; }   // cell_start, box, tile
+    // a sort binned np particles; src: the move it left to do (slot i of the new order is particle src[i])
+    void sorted(long np, const int* src) { bins_.np_binned = np; pending_src_ = src; has_bins_ = exact_ = true; esc_valid_ = false; }
+    void moved() { pending_src_ = nullptr; }               // the pending move was carried out: buf[cur] -> buf[1 - cur]
+    void pushed() { exact_ = false; esc_valid_ = true; }   // positions pushed: cells left, escapes listed
+    void held() { esc_valid_ = true; }                     // not pushed (do_not_push): nothing escaped
+    void cells_changed() { stale_ = true; }                // particles removed / appended, or the window moved them
+    void escape_list_spent() { esc_valid_ = false; }       // migration filled holes and moved tails
+
+    // the bins a collision reads must hold every particle's current cell
+    bool collision_needs_sort(long np) const { return !exact_ || bins_.np_binned != np; }
+    // the end-of-step sort is due by the interval or because the cells changed during the step; asking ends the step
+    bool end_of_step_sort_due(bool interval_due) {
+        const bool due = interval_due || (stale_ && has_bins_);
+        stale_ = false;
+        return due;
+    }
+    // migration may classify only the particles the escape list (where the species has one) names
+    bool escape_list_current() const { return esc_valid_; }
+    bool has_bins() const { return has_bins_; }
+    const pic_bins& bins() const { return bins_; }
+    const pic_bins* bins_if_sorted() const { return has_bins_ ? &bins_ : nullptr; }
+    const int* pending() const { return pending_src_; }
+private:
+    pic_bins bins_;
+    const int* pending_src_ = nullptr;
+    bool has_bins_ = false, exact_ = false, stale_ = false, esc_valid_ = false;
+};
 
 struct Species {
+    Species(double q_, double m_, const pic_bins& bins) : q(q_), m(m_), ord(bins) {}
     double q, m;
     pic_soa buf[2];        // counting sort permutes buf[cur] -> buf[1-cur]
-    int cur;
-    // A sort inside pic_engine_evolve stops at the permutation: bins describe the new order, the particles still lie
-    // in buf[cur] in the old one, and the next gather + push moves them while it reads them anyway.  Everything else
-    // that reads particle arrays calls apply_pending first; no exported call returns with a permutation pending.
-    const int* pending_src = nullptr;
-    pic_bins bins;
-    bool has_bins;
-    void* sort_work;
-    pic_escape_list esc;   // particles the last position push moved out of the domain -- over several ranks: out of
-    bool has_esc;          // the rank's brick (engine-owned)
-    bool esc_valid = false;  // the list describes the current particle order (set by the push, cleared by whatever reorders)
-    // neighbour migration (multi-rank), engine-owned device scratch
+    int cur = 0;
+    ParticleOrder ord;
+    void* sort_work = nullptr;
+    // particles the last position push moved out of the domain -- over several ranks: out of the rank's brick.  Without
+    // its memory the engine wraps with the full sweep.
+    pic_escape_list esc{};
+    DeviceBuf<int> esc_mem;      // esc.count, then esc.idx
+    bool has_esc() const { return (bool)esc_mem; }
+    // neighbour migration (multi-rank)
     long capacity = 0;           // entries of every SoA array of both buffers
     int mig_cap_max = 0, mig_cap = 0;
-    int* mig_counts = nullptr;   // [2]
-    int* mig_idx[2] = {nullptr, nullptr};
-    double* mig_msg[4] = {nullptr, nullptr, nullptr, nullptr};   // send lo/hi, recv lo/hi
-    int* mig_work = nullptr;
-    int* mig_head = nullptr;     // pinned host, 8 ints
+    DeviceBuf<int> mig_counts;   // [2]
+    DeviceBuf<int> mig_idx[2];
+    DeviceBuf<double> mig_msg[4];   // send lo/hi, recv lo/hi
+    DeviceBuf<int> mig_work;
+    PinnedBuf<int> mig_head;     // 8 ints
     // plasma injector (continuous injection behind the moving window) and absorbing boundaries
     bool has_injector = false;
     pic_plasma_injector inj{};
     double current_injection_position = 0.0;     // WarpXParticleContainer::m_current_injection_position
     uint64_t next_id = 0;
-    int* bnd_work = nullptr;     // pic_particles_boundary_workspace_ints(bnd_cap) ints, engine-owned
+    DeviceBuf<int> bnd_work;     // pic_particles_boundary_workspace_ints(bnd_cap) ints
     int bnd_cap = 0;
-    bool bins_stale = false;     // particles were removed / the window moved: re-sort before the next step
-    bool bins_exact = false;     // the bins hold every particle's current cell (set by a sort, cleared by a position push)
     // fusion reactant: the particles a fusion spent (id PIC_SPENT_ID) are listed here for the compaction, capacity + 1
-    int* spent_work = nullptr;
+    DeviceBuf<int> spent_work;
     int spent_cap = 0;
     bool do_not_push = false;      // <species>.do_not_push: x and u keep their bits (pic_engine_set_species_flags)
     bool do_not_deposit = false;   // <species>.do_not_deposit: no current deposition
@@ -77,9 +143,9 @@ struct Laser {
     pic_laser_antenna prm;
     pic_soa P;                   // borrowed device arrays, P.np particles
     long capacity;
-    int* bnd_work = nullptr;
+    DeviceBuf<int> bnd_work;
     int bnd_cap = 0;
-    double* w_owned = nullptr;   // multi-rank: weights masked to this rank's brick (engine-owned)
+    DeviceBuf<double> w_owned;   // multi-rank: weights masked to this rank's brick
 };
 
 // Per-stage CUDA-event timing of the step driver (pic_engine_enable_timing / pic_engine_stage_ms): the events are
@@ -109,7 +175,7 @@ struct Collision {
     int iprod[2] = {-1, -1};
     int type = 0;
     double multiplier = 1.0, threshold = 0.02, target = 0.002;
-    void* work = nullptr;
+    DeviceBuf<char> work;
     long pair_cap = 0;
 };
 
@@ -138,7 +204,7 @@ struct Engine {
     // With the filter the particles deposit into the engine's own copies of J and ApplyFilterJ writes from there
     // straight into the caller's arrays (no copy back): jdep[c] = fab[6 + c] with its own memory.
     pic_fab jdep[3];
-    bool jdep_alloc = false;
+    DeviceBuf<double> jdep_mem[3];
     pic_stencil st;
     pic_fab fab[9];        // Ex Ey Ez Bx By Bz jx jy jz
     std::vector<Species> species;
@@ -147,8 +213,7 @@ struct Engine {
     // multi-rank
     Comm* comm = nullptr;
     int nb[3] = {1, 1, 1}, coord[3] = {0, 0, 0};
-    double* hbuf[4] = {nullptr, nullptr, nullptr, nullptr};      // halo send lo/hi, recv lo/hi
-    size_t hbuf_doubles = 0;
+    DeviceBuf<double> hbuf[4];                   // halo send lo/hi, recv lo/hi
     // non-periodic domains
     pic_boundaries bnd{};
     bool any_pec = false, all_periodic = true;
@@ -158,16 +223,15 @@ struct Engine {
     double gamma_boost = 1.0, beta_boost = 0.0;  // warpx.gamma_boost, boost_direction = z
     bool use_nci = false;                        // particles.use_fdtd_nci_corr
     double nci_stencil[2][5];                    // [0] Ex Ey Bz, [1] Bx By Ez
-    pic_fab nci_fab[6];                          // filtered copies of E, B (engine-owned)
-    bool nci_alloc = false;
+    pic_fab nci_fab[6];                          // filtered copies of E, B
+    DeviceBuf<double> nci_mem[6];
     double cur_time = 0.0;                       // t_new[0]
-    double* shift_tmp = nullptr;                 // one component-sized scratch array
-    size_t shift_tmp_bytes = 0;
-    int* host_count = nullptr;                   // pinned host int (particles lost per boundary pass)
+    DeviceBuf<double> shift_tmp;                 // one component-sized scratch array
+    PinnedBuf<int> host_count;                   // particles removed per container and pass, one per container + 1
     std::vector<Laser> lasers;
     std::vector<Fluid> fluids;
     std::vector<Collision> collisions;
-    int* coll_status = nullptr;                  // device int: a cell exceeded the collision kernel's capacity
+    DeviceBuf<int> coll_status;                  // a cell exceeded the collision kernel's capacity
 };
 
 struct Stage {      // records the events of one stage when timing is on
@@ -212,24 +276,12 @@ static bool has_neighbour(const Engine& e, int dim, int side) {
 
 #define ENG_NCCL(x) do { if (int rc_ = (x)) return nccl_fail("pic_engine", rc_); } while (0)
 
-// Low/high neighbour exchange along one axis.  A message travelling upwards (sent to hi, received
-// from lo) is posted first on both sides: with two bricks per axis both neighbours are the same
-// rank and NCCL matches sends and receives of a pair of ranks in posting order.
+// Low/high neighbour exchange along one axis; along a non-periodic axis the bricks at the domain faces skip the
+// missing side.  A message travelling upwards (sent to hi, received from lo) is posted first on both sides: with two
+// bricks per axis both neighbours are the same rank and NCCL matches sends and receives of a pair of ranks in
+// posting order.
 static int exchange(Engine& e, int dim, const double* s_lo, const double* s_hi, double* r_lo, double* r_hi,
                     size_t n, cudaStream_t s) {
-    const int lo = neighbour(e, dim, 0), hi = neighbour(e, dim, 1);
-    ENG_NCCL(g_nccl.GroupStart());
-    ENG_NCCL(g_nccl.Send(s_hi, n, PIC_NCCL_FLOAT64, hi, e.comm->comm, s));
-    ENG_NCCL(g_nccl.Recv(r_lo, n, PIC_NCCL_FLOAT64, lo, e.comm->comm, s));
-    ENG_NCCL(g_nccl.Send(s_lo, n, PIC_NCCL_FLOAT64, lo, e.comm->comm, s));
-    ENG_NCCL(g_nccl.Recv(r_hi, n, PIC_NCCL_FLOAT64, hi, e.comm->comm, s));
-    ENG_NCCL(g_nccl.GroupEnd());
-    return 0;
-}
-
-// The same exchange along a NON-periodic axis: the bricks at the domain faces skip the missing side.
-static int exchange_np(Engine& e, int dim, const double* s_lo, const double* s_hi, double* r_lo, double* r_hi,
-                       size_t n, cudaStream_t s) {
     const bool hl = has_neighbour(e, dim, 0), hh = has_neighbour(e, dim, 1);
     const int lo = neighbour(e, dim, 0), hi = neighbour(e, dim, 1);
     ENG_NCCL(g_nccl.GroupStart());
@@ -298,19 +350,11 @@ static void lower_corner(const Engine& e, const int ng[3], double xyzmin[3], int
 
 #define ENG_CALL(x) do { if (int rc_ = (x)) return rc_; } while (0)
 
-// The four halo message buffers hold at least n doubles each.  A failed allocation leaves the engine without
-// buffers (size 0, null pointers) instead of dangling ones: a later sweep allocates again or fails cleanly.
+// The four halo message buffers hold at least n doubles each.  A failed allocation leaves that buffer empty: a later
+// sweep allocates again or fails cleanly.
 static int grow_halo_buffers(Engine& e, size_t n) {
-    if (n <= e.hbuf_doubles) return 0;
-    e.hbuf_doubles = 0;
-    for (int b = 0; b < 4; ++b) { if (e.hbuf[b]) cudaFree(e.hbuf[b]); e.hbuf[b] = nullptr; }
-    for (int b = 0; b < 4; ++b)
-        if (cudaMalloc(&e.hbuf[b], sizeof(double) * n) != cudaSuccess) {
-            cudaGetLastError();
-            for (int c = 0; c < 4; ++c) { if (e.hbuf[c]) cudaFree(e.hbuf[c]); e.hbuf[c] = nullptr; }
-            return fail("pic_engine: halo buffer allocation failed");
-        }
-    e.hbuf_doubles = n;
+    for (auto& b : e.hbuf)
+        if (b.bytes() < sizeof(double) * n) ENG_CALL(b.alloc(sizeof(double) * n, "pic_engine: halo buffer allocation failed"));
     return 0;
 }
 
@@ -332,16 +376,16 @@ static int halo_sweep(Engine& e, const pic_fab* fabs, int nfab, int dim, int ng,
             if (!has_neighbour(e, dim, side)) continue;
             size_t off = 0;
             for (int c = 0; c < nfab; ++c) {
-                ENG_CALL(pic_halo_pack(&fabs[c], dim, side, ng, mode, e.hbuf[side] + off, s));
+                ENG_CALL(pic_halo_pack(&fabs[c], dim, side, ng, mode, e.hbuf[side].get() + off, s));
                 off += (size_t)pic_halo_slab_count(&fabs[c], dim, ng, mode);
             }
         }
-        ENG_CALL(exchange_np(e, dim, e.hbuf[0], e.hbuf[1], e.hbuf[2], e.hbuf[3], n, (cudaStream_t)s));
+        ENG_CALL(exchange(e, dim, e.hbuf[0].get(), e.hbuf[1].get(), e.hbuf[2].get(), e.hbuf[3].get(), n, (cudaStream_t)s));
         for (int side = 0; side < 2; ++side) {
             if (!has_neighbour(e, dim, side)) continue;
             size_t off = 0;
             for (int c = 0; c < nfab; ++c) {
-                ENG_CALL(pic_halo_unpack(&fabs[c], dim, side, ng, mode, e.hbuf[2 + side] + off, s));
+                ENG_CALL(pic_halo_unpack(&fabs[c], dim, side, ng, mode, e.hbuf[2 + side].get() + off, s));
                 off += (size_t)pic_halo_slab_count(&fabs[c], dim, ng, mode);
             }
         }
@@ -356,9 +400,9 @@ static int halo_sweep(Engine& e, const pic_fab* fabs, int nfab, int dim, int ng,
     size_t n = 0;
     for (int c = 0; c < nfab; ++c) n += (size_t)pic_halo_slab_count(&fabs[c], dim, ng, mode);
     ENG_CALL(grow_halo_buffers(e, n));
-    ENG_CALL(pic_halo_pack_multi(fabs, nfab, dim, ng, mode, e.hbuf[0], e.hbuf[1], s));
-    ENG_CALL(exchange(e, dim, e.hbuf[0], e.hbuf[1], e.hbuf[2], e.hbuf[3], n, (cudaStream_t)s));
-    ENG_CALL(pic_halo_unpack_multi(fabs, nfab, dim, ng, mode, e.hbuf[2], e.hbuf[3], s));
+    ENG_CALL(pic_halo_pack_multi(fabs, nfab, dim, ng, mode, e.hbuf[0].get(), e.hbuf[1].get(), s));
+    ENG_CALL(exchange(e, dim, e.hbuf[0].get(), e.hbuf[1].get(), e.hbuf[2].get(), e.hbuf[3].get(), n, (cudaStream_t)s));
+    ENG_CALL(pic_halo_unpack_multi(fabs, nfab, dim, ng, mode, e.hbuf[2].get(), e.hbuf[3].get(), s));
     return 0;
 }
 
@@ -395,10 +439,10 @@ static int sync_current(Engine& e, void* s) {
 
 // the move a deferred sort left out: buf[cur] -> buf[1-cur] through the permutation
 static int apply_pending(Species& sp, void* s) {
-    if (!sp.pending_src) return 0;
-    ENG_CALL(pic_sort_apply_permutation(&sp.buf[sp.cur], &sp.buf[1 - sp.cur], sp.pending_src, s));
+    if (!sp.ord.pending()) return 0;
+    ENG_CALL(pic_sort_apply_permutation(&sp.buf[sp.cur], &sp.buf[1 - sp.cur], sp.ord.pending(), s));
     sp.cur = 1 - sp.cur;
-    sp.pending_src = nullptr;
+    sp.ord.moved();
     return 0;
 }
 
@@ -407,10 +451,10 @@ static int push(Engine& e, Species& sp, double dt, int push_position, void* s) {
     lower_corner(e, e.ng_EB, xyzmin, lo);
     // only the default supercell kernel of PushPX carries a pending sort; PushP, order 4 and the pair kernels get the
     // particles moved first
-    if (!(push_position && sp.has_bins && e.nox <= 3 && g_gather_mode == PIC_GATHER_TILE)) ENG_CALL(apply_pending(sp, s));
+    if (!(push_position && sp.ord.has_bins() && gather_push_carries_permutation(e.nox))) ENG_CALL(apply_pending(sp, s));
     const pic_soa& P = sp.buf[sp.cur];
-    if (push_position) sp.bins_exact = false;
-    if (push_position && sp.has_esc) {
+    if (push_position) sp.ord.pushed();
+    if (push_position && sp.has_esc()) {
         cudaMemsetAsync(sp.esc.count, 0, sizeof(int), (cudaStream_t)s);
         // Over several ranks the push lists what leaves the BRICK (a superset by 1e-6 cell, so that round-off at a face
         // cannot hide a particle from the classification, which decides by cell index): the periodic wrap and the
@@ -425,33 +469,38 @@ static int push(Engine& e, Species& sp, double dt, int push_position, void* s) {
                 sp.esc.hi[d] = e.geom.periodic[d] ? e.geom.prob_hi[d] : INFINITY;
             }
         }
-        sp.esc_valid = true;
     }
     // the main push gathers from the NCI-filtered copies (PhysicalParticleContainer.cpp:1900-1911); PushP does not
     const pic_fab* EB = (e.use_nci && push_position) ? e.nci_fab : e.fab;
-    if (sp.pending_src) {
-        const int* src = sp.pending_src;
-        sp.pending_src = nullptr;
+    if (const int* src = sp.ord.pending()) {
+        sp.ord.moved();
         sp.cur = 1 - sp.cur;
         return pic_gather_push_permuted(&P, &sp.buf[sp.cur], src, &EB[0], &EB[3], e.dinv, xyzmin, lo, sp.q, sp.m, dt, e.nox,
-                                        e.galerkin, e.pusher, &sp.bins, sp.has_esc ? &sp.esc : nullptr, s);
+                                        e.galerkin, e.pusher, &sp.ord.bins(), sp.has_esc() ? &sp.esc : nullptr, s);
     }
     return pic_gather_push(&P, 0, P.np, &EB[0], &EB[3], e.dinv, xyzmin, lo, sp.q, sp.m, dt, e.nox,
-                           e.galerkin, e.pusher, push_position, sp.has_bins ? &sp.bins : nullptr,
-                           sp.has_esc ? &sp.esc : nullptr, s);
+                           e.galerkin, e.pusher, push_position, sp.ord.bins_if_sorted(),
+                           sp.has_esc() ? &sp.esc : nullptr, s);
+}
+
+// Engine-owned copies of n field components with the shapes of src (the NCI-filtered E, B; the deposition copy of J):
+// either all n are allocated or none.
+static int alloc_fab_copies(const pic_fab* src, int n, pic_fab* copy, DeviceBuf<double>* mem, const char* what) {
+    DeviceBuf<double> m[6];
+    for (int c = 0; c < n; ++c) ENG_CALL(m[c].alloc(sizeof(double) * (size_t)fab_size(src[c]), what));
+    for (int c = 0; c < n; ++c) {
+        mem[c] = std::move(m[c]);
+        copy[c] = src[c];
+        copy[c].p = mem[c].get();
+    }
+    return 0;
 }
 
 // PhysicalParticleContainer::applyNCIFilter for the rank's box (one tile): E, B -> the engine's filtered copies
 static int apply_nci(Engine& e, void* s) {
-    if (!e.nci_alloc) {
-        for (int c = 0; c < 6; ++c) {
-            e.nci_fab[c] = e.fab[c];
-            e.nci_fab[c].p = nullptr;
-            if (cudaMalloc(&e.nci_fab[c].p, sizeof(double) * (size_t)fab_size(e.fab[c])) != cudaSuccess)
-                return fail("pic_engine: cannot allocate the NCI-filtered field copies");
-            cudaMemsetAsync(e.nci_fab[c].p, 0, sizeof(double) * (size_t)fab_size(e.fab[c]), (cudaStream_t)s);
-        }
-        e.nci_alloc = true;
+    if (!e.nci_mem[0]) {
+        ENG_CALL(alloc_fab_copies(e.fab, 6, e.nci_fab, e.nci_mem, "pic_engine: cannot allocate the NCI-filtered field copies"));
+        for (int c = 0; c < 6; ++c) cudaMemsetAsync(e.nci_fab[c].p, 0, e.nci_mem[c].bytes(), (cudaStream_t)s);
     }
     for (int c = 0; c < 6; ++c) {
         const bool exeybz = (c == 0 || c == 1 || c == 5);              // :2132-2163
@@ -464,10 +513,8 @@ static int apply_nci(Engine& e, void* s) {
 // + push, and its escape list is empty -- nothing left the domain or the brick.  Its bins stay exact.
 static int hold(Species& sp, void* s) {
     ENG_CALL(apply_pending(sp, s));
-    if (sp.has_esc) {
-        cudaMemsetAsync(sp.esc.count, 0, sizeof(int), (cudaStream_t)s);
-        sp.esc_valid = true;
-    }
+    if (sp.has_esc()) cudaMemsetAsync(sp.esc.count, 0, sizeof(int), (cudaStream_t)s);
+    sp.ord.held();
     return 0;
 }
 
@@ -481,15 +528,8 @@ static int push_particles_and_deposit(Engine& e, void* s) {
     }
     {
         Stage t(e, ST_ZERO_J, s);
-        if (e.use_filter && !e.jdep_alloc) {
-            for (int c = 0; c < 3; ++c) {
-                e.jdep[c] = e.fab[6 + c];
-                e.jdep[c].p = nullptr;
-                if (cudaMalloc(&e.jdep[c].p, sizeof(double) * (size_t)fab_size(e.fab[6 + c])) != cudaSuccess)
-                    return fail("pic_engine: cannot allocate the deposition copy of J (filter)");
-            }
-            e.jdep_alloc = true;
-        }
+        if (e.use_filter && !e.jdep_mem[0])
+            ENG_CALL(alloc_fab_copies(&e.fab[6], 3, e.jdep, e.jdep_mem, "pic_engine: cannot allocate the deposition copy of J (filter)"));
         const pic_fab* Jd = e.use_filter ? e.jdep : &e.fab[6];
         for (int c = 0; c < 3; ++c)                     // J.setVal(0), MultiParticleContainer.cpp:467-478
             cudaMemsetAsync(Jd[c].p, 0, sizeof(double) * (size_t)fab_size(Jd[c]), (cudaStream_t)s);
@@ -504,7 +544,7 @@ static int push_particles_and_deposit(Engine& e, void* s) {
         const pic_soa& P = sp.buf[sp.cur];
         Stage t(e, ST_DEPOSIT, s);
         ENG_CALL(pic_deposit_esirkepov(&P, 0, P.np, Jd, e.dinv, xyzmin, lo, sp.q, e.dt, -0.5 * e.dt,
-                                       e.nox, sp.has_bins ? &sp.bins : nullptr, s));
+                                       e.nox, sp.ord.bins_if_sorted(), s));
     }
     // the antennas come after the species in allcontainers (MultiParticleContainer.cpp:60-75);
     // LaserParticleContainer::Evolve (:563-700): push at t^n, deposit with charge = 1 (:88)
@@ -520,8 +560,8 @@ static int push_particles_and_deposit(Engine& e, void* s) {
                 own_lo[d] = (e.nb[d] == 1 || !has_neighbour(e, d, 0)) ? -INFINITY : e.geom.prob_lo[d] + e.dx[d] * e.box_lo[d];
                 own_hi[d] = (e.nb[d] == 1 || !has_neighbour(e, d, 1)) ? INFINITY : e.geom.prob_lo[d] + e.dx[d] * (e.box_hi[d] + 1);
             }
-            ENG_CALL(pic_particles_owned_weights(&L.P, own_lo, own_hi, L.w_owned, s));
-            dep.w = L.w_owned;
+            ENG_CALL(pic_particles_owned_weights(&L.P, own_lo, own_hi, L.w_owned.get(), s));
+            dep.w = L.w_owned.get();
         }
         ENG_CALL(pic_deposit_esirkepov(&dep, 0, dep.np, Jd, e.dinv, xyzmin, lo, 1.0, e.dt, -0.5 * e.dt,
                                        e.nox, nullptr, s));
@@ -529,17 +569,14 @@ static int push_particles_and_deposit(Engine& e, void* s) {
     return 0;
 }
 
-// defer: leave the move to the next gather + push (sp.pending_src)
+// defer: leave the move to the next gather + push (sp.ord.pending())
 static int sort_species(Engine& e, Species& sp, bool defer, void* s) {
     ENG_CALL(apply_pending(sp, s));
     pic_soa& in = sp.buf[sp.cur];
     sp.buf[1 - sp.cur].np = in.np;
-    for (int d = 0; d < 3; ++d) { sp.bins.box_lo[d] = e.box_lo[d]; sp.bins.box_hi[d] = e.box_hi[d]; }
-    ENG_CALL(pic_sort_index_by_cell(&in, &e.geom, &sp.bins, sp.sort_work, &sp.pending_src, s));
-    sp.bins.np_binned = in.np;
-    sp.has_bins = true;
-    sp.bins_exact = true;
-    sp.esc_valid = false;
+    const int* src = nullptr;
+    ENG_CALL(pic_sort_index_by_cell(&in, &e.geom, &sp.ord.bins(), sp.sort_work, &src, s));
+    sp.ord.sorted(in.np, src);
     return defer ? 0 : apply_pending(sp, s);
 }
 
@@ -561,47 +598,48 @@ static int migrate(Engine& e, Species& sp, void* stream) {
     pic_soa& P = sp.buf[sp.cur];
     const int cap = sp.mig_cap;
     const size_t nmsg = (size_t)pic_migrate_message_doubles(cap);
-    for (int n = 0; n < 8; ++n) sp.mig_head[n] = 0;
-    sp.mig_head[0] = (int)P.np;
-    cudaMemcpyAsync(sp.mig_work, sp.mig_head, 8 * sizeof(int), cudaMemcpyHostToDevice, s);
-    const int* np_dev = sp.mig_work;
+    int* head = sp.mig_head.get();
+    int* work = sp.mig_work.get();
+    int* counts = sp.mig_counts.get();
+    int* idx[2] = {sp.mig_idx[0].get(), sp.mig_idx[1].get()};
+    double* msg[4] = {sp.mig_msg[0].get(), sp.mig_msg[1].get(), sp.mig_msg[2].get(), sp.mig_msg[3].get()};
+    for (int n = 0; n < 8; ++n) head[n] = 0;
+    head[0] = (int)P.np;
+    cudaMemcpyAsync(work, head, 8 * sizeof(int), cudaMemcpyHostToDevice, s);
+    const int* np_dev = work;
     pic_soa view = P;
     view.np = sp.capacity;                       // launch bound only: the kernels read the count from np_dev
     // Who can leave: the particles the push of this step listed (nothing else moved since: periodic particle boundaries
     // remove nobody, no window shift re-drew the brick) -- else every particle is classified.
-    const bool listed = sp.has_esc && sp.esc_valid && e.all_periodic && !e.do_moving_window && !g_migrate_full_sweep;
+    const bool listed = sp.has_esc() && sp.ord.escape_list_current() && e.all_periodic && !e.do_moving_window &&
+                        !g_migrate_full_sweep;
     for (int dim = 0; dim < 3; ++dim) {
         if (spans(e, dim)) continue;
         const bool np_dim = !e.geom.periodic[dim];
         if (listed) ++g_listed_sweeps;
         if (listed)
             ENG_CALL(pic_particles_classify_listed(&view, &e.geom, dim, e.box_lo[dim], e.box_hi[dim],
-                                                   np_dim ? 2 : (e.nb[dim] == 2 ? 1 : 0), sp.mig_counts, sp.mig_idx[0],
-                                                   sp.mig_idx[1], cap, np_dev, &sp.esc, s));
+                                                   np_dim ? 2 : (e.nb[dim] == 2 ? 1 : 0), counts, idx[0], idx[1], cap,
+                                                   np_dev, &sp.esc, s));
         else
         ENG_CALL(pic_particles_classify(&view, &e.geom, dim, e.box_lo[dim], e.box_hi[dim],
-                                        np_dim ? 2 : (e.nb[dim] == 2 ? 1 : 0),
-                                        sp.mig_counts, sp.mig_idx[0], sp.mig_idx[1], cap, np_dev, s));
-        peak_kernel<<<1, 1, 0, s>>>(sp.mig_work + 6, sp.mig_counts);
+                                        np_dim ? 2 : (e.nb[dim] == 2 ? 1 : 0), counts, idx[0], idx[1], cap, np_dev, s));
+        peak_kernel<<<1, 1, 0, s>>>(work + 6, counts);
         count_launch();
-        ENG_CALL(pic_migrate_pack(&view, sp.mig_idx[0], sp.mig_counts, cap, sp.mig_msg[0], s));
-        ENG_CALL(pic_migrate_pack(&view, sp.mig_idx[1], sp.mig_counts + 1, cap, sp.mig_msg[1], s));
-        if (np_dim) {
-            // a missing neighbour sends nothing: its message reads "0 particles"
-            for (int side = 0; side < 2; ++side)
-                if (!has_neighbour(e, dim, side)) cudaMemsetAsync(sp.mig_msg[2 + side], 0, sizeof(double), s);
-            ENG_CALL(exchange_np(e, dim, sp.mig_msg[0], sp.mig_msg[1], sp.mig_msg[2], sp.mig_msg[3], nmsg, s));
-        } else
-        ENG_CALL(exchange(e, dim, sp.mig_msg[0], sp.mig_msg[1], sp.mig_msg[2], sp.mig_msg[3], nmsg, s));
-        ENG_CALL(pic_migrate_unpack(&view, sp.mig_counts, sp.mig_idx[0], sp.mig_idx[1], sp.mig_msg[2], sp.mig_msg[3], cap,
-                                    sp.capacity, sp.mig_work, np_dev, s));
-        if (listed) ENG_CALL(pic_migrate_note_appended(sp.mig_work, &sp.esc, s));     // arrivals may have to travel on
+        ENG_CALL(pic_migrate_pack(&view, idx[0], counts, cap, msg[0], s));
+        ENG_CALL(pic_migrate_pack(&view, idx[1], counts + 1, cap, msg[1], s));
+        // a missing neighbour (beyond a non-periodic face) sends nothing: its message reads "0 particles"
+        for (int side = 0; side < 2; ++side)
+            if (!has_neighbour(e, dim, side)) cudaMemsetAsync(msg[2 + side], 0, sizeof(double), s);
+        ENG_CALL(exchange(e, dim, msg[0], msg[1], msg[2], msg[3], nmsg, s));
+        ENG_CALL(pic_migrate_unpack(&view, counts, idx[0], idx[1], msg[2], msg[3], cap, sp.capacity, work, np_dev, s));
+        if (listed) ENG_CALL(pic_migrate_note_appended(work, &sp.esc, s));     // arrivals may have to travel on
     }
-    sp.esc_valid = false;            // holes were filled, tails moved: the list is spent
-    ENG_NCCL(g_nccl.AllReduce(sp.mig_work + 6, sp.mig_work + 6, 1, PIC_NCCL_INT32, PIC_NCCL_MAX, e.comm->comm, s));
-    cudaMemcpyAsync(sp.mig_head, sp.mig_work, 8 * sizeof(int), cudaMemcpyDeviceToHost, s);
+    sp.ord.escape_list_spent();
+    ENG_NCCL(g_nccl.AllReduce(work + 6, work + 6, 1, PIC_NCCL_INT32, PIC_NCCL_MAX, e.comm->comm, s));
+    cudaMemcpyAsync(head, work, 8 * sizeof(int), cudaMemcpyDeviceToHost, s);
     if (cudaStreamSynchronize(s) != cudaSuccess) return fail("pic_engine: migration failed (%s)", cudaGetErrorString(cudaGetLastError()));
-    const int np_new = sp.mig_head[0], status = sp.mig_head[1], seen = sp.mig_head[6];
+    const int np_new = head[0], status = head[1], seen = head[6];
     if (status)
         return fail("pic_engine: particle migration overflow on rank %d (status %d, %d particles through one face, "
                     "message capacity %d, tile capacity %ld)", e.comm->rank, status, seen, cap, sp.capacity);
@@ -630,12 +668,8 @@ static int evolve_e(Engine& e, double dt, void* s) {
 
 static int shift_component(Engine& e, int c, int num_shift, void* s) {
     const size_t bytes = sizeof(double) * (size_t)fab_size(e.fab[c]);
-    if (bytes > e.shift_tmp_bytes) {
-        if (e.shift_tmp) cudaFree(e.shift_tmp);
-        if (cudaMalloc(&e.shift_tmp, bytes) != cudaSuccess) return fail("pic_engine: moving-window scratch allocation failed");
-        e.shift_tmp_bytes = bytes;
-    }
-    return pic_shift_fab(&e.fab[c], e.shift_tmp, &e.geom, num_shift, e.mw_dir, 0.0 /* no external field */, s);
+    if (bytes > e.shift_tmp.bytes()) ENG_CALL(e.shift_tmp.alloc(bytes, "pic_engine: moving-window scratch allocation failed"));
+    return pic_shift_fab(&e.fab[c], e.shift_tmp.get(), &e.geom, num_shift, e.mw_dir, 0.0 /* no external field */, s);
 }
 
 // WarpX::MoveWindow (Utils/WarpXMovingWindow.cpp:139-476), one level, lab or z-boosted frame, no PML: advance
@@ -697,39 +731,47 @@ static int move_window(Engine& e, bool move_j, int* num_moved, void* s) {
             sp.current_injection_position = new_pos;
         }
     }
-    for (auto& sp : e.species) sp.bins_stale = true;     // every particle changed cell along dir
+    for (auto& sp : e.species) sp.ord.cells_changed();     // every particle changed cell along dir
     *num_moved = nsb;
     return 0;
 }
 
-// mypc->ApplyBoundaryConditions() over species and lasers (MultiParticleContainer.cpp:659-664) and the
-// removal AMReX Redistribute performs: all marks first, ONE host read of the counts, then the compactions.
+// One particle container of a removal pass (a species, or an antenna when sp is null) and the workspace its marks go to
+struct Removal {
+    Species* sp; Laser* L; int* work; int cap;
+    pic_soa& P() const { return sp ? sp->buf[sp->cur] : L->P; }
+};
+
+// The removal AMReX Redistribute performs: mark(r) lists the particles of every container r to remove (work[0] = how
+// many), ONE host read of the counts, then the compactions.
+template <class Mark>
+static int remove_marked(Engine& e, const std::vector<Removal>& rs, Mark mark, const char* pass, cudaStream_t s) {
+    if (rs.empty()) return 0;
+    for (size_t n = 0; n < rs.size(); ++n) {
+        ENG_CALL(mark(rs[n]));
+        cudaMemcpyAsync(e.host_count.get() + n, rs[n].work, sizeof(int), cudaMemcpyDeviceToHost, s);
+    }
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail("pic_engine: %s failed (%s)", pass, cudaGetErrorString(cudaGetLastError()));
+    for (size_t n = 0; n < rs.size(); ++n) {
+        const int lost = e.host_count.get()[n];
+        if (lost == 0) continue;
+        pic_soa& P = rs[n].P();
+        ENG_CALL(pic_particles_boundary_compact(&P, rs[n].work, rs[n].cap, lost, s));
+        P.np -= lost;
+        if (rs[n].sp) rs[n].sp->ord.cells_changed();
+    }
+    return 0;
+}
+
+// mypc->ApplyBoundaryConditions() over species and lasers (MultiParticleContainer.cpp:659-664) and the removal
 static int apply_particle_boundaries(Engine& e, void* stream) {
     if (e.all_periodic) return 0;
     cudaStream_t s = (cudaStream_t)stream;
-    const size_t nsp = e.species.size(), ncont = nsp + e.lasers.size();
-    if (ncont == 0) return 0;
-    for (size_t n = 0; n < ncont; ++n) {
-        const bool is_sp = n < nsp;
-        pic_soa& P = is_sp ? e.species[n].buf[e.species[n].cur] : e.lasers[n - nsp].P;
-        int* work = is_sp ? e.species[n].bnd_work : e.lasers[n - nsp].bnd_work;
-        const int cap = is_sp ? e.species[n].bnd_cap : e.lasers[n - nsp].bnd_cap;
-        ENG_CALL(pic_particles_boundary_mark(&P, &e.geom, &e.bnd, work, cap, s));
-        cudaMemcpyAsync(e.host_count + n, work, sizeof(int), cudaMemcpyDeviceToHost, s);
-    }
-    if (cudaStreamSynchronize(s) != cudaSuccess) return fail("pic_engine: particle boundary pass failed (%s)", cudaGetErrorString(cudaGetLastError()));
-    for (size_t n = 0; n < ncont; ++n) {
-        const int lost = e.host_count[n];
-        if (lost == 0) continue;
-        const bool is_sp = n < nsp;
-        pic_soa& P = is_sp ? e.species[n].buf[e.species[n].cur] : e.lasers[n - nsp].P;
-        int* work = is_sp ? e.species[n].bnd_work : e.lasers[n - nsp].bnd_work;
-        const int cap = is_sp ? e.species[n].bnd_cap : e.lasers[n - nsp].bnd_cap;
-        ENG_CALL(pic_particles_boundary_compact(&P, work, cap, lost, s));
-        P.np -= lost;
-        if (is_sp) e.species[n].bins_stale = true;
-    }
-    return 0;
+    std::vector<Removal> rs;
+    for (auto& sp : e.species) rs.push_back({&sp, nullptr, sp.bnd_work.get(), sp.bnd_cap});
+    for (auto& L : e.lasers) rs.push_back({nullptr, &L, L.bnd_work.get(), L.bnd_cap});
+    return remove_marked(e, rs, [&](const Removal& r) { return pic_particles_boundary_mark(&r.P(), &e.geom, &e.bnd, r.work, r.cap, s); },
+                         "particle boundary pass", s);
 }
 
 // WarpXFluidContainer::Evolve (Source/Fluids/WarpXFluidContainer.cpp:257-314) on a periodic domain: GatherAndPush,
@@ -749,29 +791,37 @@ static int evolve_fluid(Engine& e, Fluid& fl, void* s) {
 // at t_new: a collision runs when int(floor(t / dt)) % ndt == 0, with dt * ndt.  Its species need their current cells:
 // one not sorted since its last position push (or with particles appended behind the bins) is sorted here first, with
 // the move left to this step's gather + push like the end-of-step sort.
+// The parameters pic_coulomb_collision and pic_fusion_collision share, for entry ic of the collisions
+template <class Prm>
+static Prm pair_params(const Collision& c, int ic, Species* const sp[2]) {
+    Prm p{};
+    p.q1 = sp[0]->q; p.m1 = sp[0]->m; p.q2 = sp[1]->q; p.m2 = sp[1]->m;
+    p.seed = c.seed; p.collision_index = ic; p.same_species = c.isp1 == c.isp2 ? 1 : 0;
+    return p;
+}
+// the part of a colliding species' sort workspace that is free until its next sort
+static int* sort_scratch(const Species& sp) { return pic_sort_scratch(sp.sort_work, sp.ord.bins().np_binned); }
+
 static int do_fusion(Engine& e, const Collision& c, int ic, Species* sp[2], void* s) {
-    pic_fusion_collision fc;
-    fc.q1 = sp[0]->q; fc.m1 = sp[0]->m; fc.q2 = sp[1]->q; fc.m2 = sp[1]->m;
+    pic_fusion_collision fc = pair_params<pic_fusion_collision>(c, ic, sp);
     const bool pb = c.type == PIC_FUSION_PB_3HE4;      // one product species: six alphas per event
     Species* pr[2] = {&e.species[c.iprod[0]], pb ? nullptr : &e.species[c.iprod[1]]};
     fc.mA = pr[0]->m; fc.mB = pb ? 0.0 : pr[1]->m;
     fc.type = c.type; fc.fusion_multiplier = c.multiplier;
     fc.fusion_probability_threshold = c.threshold; fc.fusion_probability_target_value = c.target;
-    fc.seed = c.seed; fc.collision_index = ic; fc.same_species = c.isp1 == c.isp2 ? 1 : 0;
     {
         Stage t(e, ST_FUSION, s);
-        ENG_CALL(pic_collide_nuclear_fusion(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, sp[0]->pending_src,
-                                            &sp[1]->buf[sp[1]->cur], &sp[1]->bins, sp[1]->pending_src, &e.geom,
-                                            e.dt * c.ndt, e.istep, pic_sort_scratch(sp[0]->sort_work, sp[0]->bins.np_binned),
-                                            pic_sort_scratch(sp[1]->sort_work, sp[1]->bins.np_binned), c.work, c.pair_cap,
-                                            e.coll_status, s));
+        ENG_CALL(pic_collide_nuclear_fusion(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->ord.bins(), sp[0]->ord.pending(),
+                                            &sp[1]->buf[sp[1]->cur], &sp[1]->ord.bins(), sp[1]->ord.pending(), &e.geom,
+                                            e.dt * c.ndt, e.istep, sort_scratch(*sp[0]), sort_scratch(*sp[1]), c.work.get(),
+                                            c.pair_cap, e.coll_status.get(), s));
     }
     Stage t(e, ST_FUSION_PRODUCTS, s);
     for (Species* p : pr)                // products are appended behind the particles in place
         if (p) ENG_CALL(apply_pending(*p, s));
     long nev = 0;
-    ENG_CALL(pic_fusion_create_products(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, &sp[1]->buf[sp[1]->cur],
-                                        &sp[1]->bins, &e.geom, e.istep, c.work, c.pair_cap, &pr[0]->buf[pr[0]->cur],
+    ENG_CALL(pic_fusion_create_products(&fc, &sp[0]->buf[sp[0]->cur], &sp[0]->ord.bins(), &sp[1]->buf[sp[1]->cur],
+                                        &sp[1]->ord.bins(), &e.geom, e.istep, c.work.get(), c.pair_cap, &pr[0]->buf[pr[0]->cur],
                                         pr[0]->capacity, pr[0]->next_id, pb ? nullptr : &pr[1]->buf[pr[1]->cur],
                                         pb ? 0 : pr[1]->capacity, pb ? 0 : pr[1]->next_id, &nev, s));
     const long per_event = pb ? 6 : 2;
@@ -779,7 +829,7 @@ static int do_fusion(Engine& e, const Collision& c, int ic, Species* sp[2], void
         if (!p) continue;
         p->buf[p->cur].np += per_event * nev;
         p->next_id += (uint64_t)(per_event * nev);
-        if (nev) p->bins_stale = true;
+        if (nev) p->ord.cells_changed();
     }
     return 0;
 }
@@ -790,48 +840,33 @@ static int do_collisions(Engine& e, void* s) {
         if (int(std::floor(e.cur_time / e.dt)) % c.ndt != 0) continue;
         Species* sp[2] = {&e.species[c.isp1], &e.species[c.isp2]};
         for (Species* p : sp)
-            if (!p->bins_exact || p->bins.np_binned != p->buf[p->cur].np) {
+            if (p->ord.collision_needs_sort(p->buf[p->cur].np)) {
                 Stage t(e, ST_SORT, s);
                 ENG_CALL(sort_species(e, *p, true, s));
             }
         if (c.fusion) { ENG_CALL(do_fusion(e, c, (int)ic, sp, s)); continue; }
         Stage t(e, ST_COLLISIONS, s);
-        pic_coulomb_collision cc;
-        cc.q1 = sp[0]->q; cc.m1 = sp[0]->m; cc.q2 = sp[1]->q; cc.m2 = sp[1]->m;
-        cc.coulomb_log = c.coulomb_log; cc.seed = c.seed; cc.collision_index = (int)ic;
-        cc.same_species = c.isp1 == c.isp2 ? 1 : 0;
-        ENG_CALL(pic_collide_pairwise_coulomb(&cc, &sp[0]->buf[sp[0]->cur], &sp[0]->bins, sp[0]->pending_src,
-                                              &sp[1]->buf[sp[1]->cur], &sp[1]->bins, sp[1]->pending_src, &e.geom,
-                                              e.dt * c.ndt, e.istep, pic_sort_scratch(sp[0]->sort_work, sp[0]->bins.np_binned),
-                                              pic_sort_scratch(sp[1]->sort_work, sp[1]->bins.np_binned), e.coll_status, s));
+        pic_coulomb_collision cc = pair_params<pic_coulomb_collision>(c, (int)ic, sp);
+        cc.coulomb_log = c.coulomb_log;
+        ENG_CALL(pic_collide_pairwise_coulomb(&cc, &sp[0]->buf[sp[0]->cur], &sp[0]->ord.bins(), sp[0]->ord.pending(),
+                                              &sp[1]->buf[sp[1]->cur], &sp[1]->ord.bins(), sp[1]->ord.pending(), &e.geom,
+                                              e.dt * c.ndt, e.istep, sort_scratch(*sp[0]), sort_scratch(*sp[1]),
+                                              e.coll_status.get(), s));
     }
     return 0;
 }
 
 // The reactants a fusion spent leave with the particles lost at the boundaries (the reference's
-// deleteInvalidParticles, BinaryCollision.H:212-218): all marks, ONE host read of the counts, the compactions.
+// deleteInvalidParticles, BinaryCollision.H:212-218), in a pass of their own: the marks must see the compacted arrays.
 static int remove_spent(Engine& e, void* stream) {
     cudaStream_t s = (cudaStream_t)stream;
-    bool any = false;
-    for (size_t n = 0; n < e.species.size(); ++n) {
-        Species& sp = e.species[n];
-        if (!sp.spent_work) continue;
-        ENG_CALL(apply_pending(sp, s));
-        ENG_CALL(pic_particles_mark_spent(&sp.buf[sp.cur], sp.spent_work, sp.spent_cap, s));
-        cudaMemcpyAsync(e.host_count + n, sp.spent_work, sizeof(int), cudaMemcpyDeviceToHost, s);
-        any = true;
-    }
-    if (!any) return 0;
-    if (cudaStreamSynchronize(s) != cudaSuccess) return fail("pic_engine: spent-reactant pass failed (%s)", cudaGetErrorString(cudaGetLastError()));
-    for (size_t n = 0; n < e.species.size(); ++n) {
-        Species& sp = e.species[n];
-        if (!sp.spent_work || e.host_count[n] == 0) continue;
-        pic_soa& P = sp.buf[sp.cur];
-        ENG_CALL(pic_particles_boundary_compact(&P, sp.spent_work, sp.spent_cap, e.host_count[n], s));
-        P.np -= e.host_count[n];
-        sp.bins_stale = true;
-    }
-    return 0;
+    std::vector<Removal> rs;
+    for (auto& sp : e.species)
+        if (sp.spent_work) rs.push_back({&sp, nullptr, sp.spent_work.get(), sp.spent_cap});
+    return remove_marked(e, rs, [&](const Removal& r) {
+        ENG_CALL(apply_pending(*r.sp, s));
+        return pic_particles_mark_spent(&r.P(), r.work, r.cap, s);
+    }, "spent-reactant pass", s);
 }
 
 // last: Synchronize() ends the step; defer_sort: another step of the same call follows, its push moves the sorted particles
@@ -882,7 +917,7 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
             // amrex enforcePeriodic: only the particles the push of this step moved out of the domain
             // (done before the removal below, while the indices listed by the push are still valid; the
             // two act on different directions)
-            if (sp.has_esc) ENG_CALL(pic_particles_wrap_listed(&sp.buf[sp.cur], &e.geom, &sp.esc, s));
+            if (sp.has_esc()) ENG_CALL(pic_particles_wrap_listed(&sp.buf[sp.cur], &e.geom, &sp.esc, s));
             else ENG_CALL(pic_particles_wrap_periodic(&sp.buf[sp.cur], &e.geom, s));
         }
         for (auto& L : e.lasers) ENG_CALL(pic_particles_wrap_periodic(&L.P, &e.geom, s));
@@ -891,9 +926,8 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     }
     for (auto& sp : e.species) {
         if (e.comm) { Stage t(e, ST_MIGRATE, s); ENG_CALL(migrate(e, sp, s)); }
-        const bool due = e.sort_interval > 0 && (step + 1) % e.sort_interval == 0;
-        if (sp.sort_work && (due || (sp.bins_stale && sp.has_bins))) { Stage t(e, ST_SORT, s); ENG_CALL(sort_species(e, sp, defer_sort, s)); }
-        sp.bins_stale = false;
+        const bool due = sp.ord.end_of_step_sort_due(e.sort_interval > 0 && (step + 1) % e.sort_interval == 0);
+        if (sp.sort_work && due) { Stage t(e, ST_SORT, s); ENG_CALL(sort_species(e, sp, defer_sort, s)); }
     }
     if (e.tm.on && e.tm.recs.size() > 4096) collect_timing(e);          // bound the event pool of long runs
     return 0;
@@ -903,8 +937,17 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
 
 using namespace pic;
 
-static int alloc_boundary_scratch(long capacity, int** work, int* cap);
-static int grow_host_counts(Engine& e);
+// The particle-boundary scratch of a container of `capacity` particles
+static int alloc_boundary_scratch(long capacity, DeviceBuf<int>& work, int* cap) {
+    const long c = capacity / 16 + 65536;
+    *cap = (int)(c < capacity + 1 ? c : capacity + 1);
+    return work.alloc(sizeof(int) * (size_t)pic_particles_boundary_workspace_ints(*cap),
+                      "pic_engine: cannot allocate the particle-boundary scratch");
+}
+// The pinned counts of the removal passes for the engine's containers and one more, plus a spare slot
+static int alloc_host_counts_for_one_more(const Engine& e, PinnedBuf<int>& counts) {
+    return counts.alloc(sizeof(int) * (e.species.size() + e.lasers.size() + 2), "pic_engine: cannot allocate pinned host memory");
+}
 
 // Defaults of the kernel-variant switches from the environment (PIC_FDTD_MODE, PIC_DEPOSIT_MODE, PIC_GATHER_MODE):
 // lets a launcher pin a variant without touching the host code.  Applied once, when the library is loaded.
@@ -945,29 +988,9 @@ extern "C" void* pic_engine_create(const pic_geom* geom, const int box_lo[3], co
 }
 extern "C" void pic_engine_destroy(void* h) {
     Engine* e = static_cast<Engine*>(h);
-    if (e && e->jdep_alloc) for (int c = 0; c < 3; ++c) cudaFree(e->jdep[c].p);
-    if (e) {
 #ifndef PIC_SIMT_HOST
-        for (cudaEvent_t ev : e->tm.pool) cudaEventDestroy(ev);
+    if (e) for (cudaEvent_t ev : e->tm.pool) cudaEventDestroy(ev);
 #endif
-        for (auto& sp : e->species) {
-            if (sp.has_esc) cudaFree(sp.esc.count);
-            if (sp.mig_counts) cudaFree(sp.mig_counts);
-            for (int b = 0; b < 2; ++b) if (sp.mig_idx[b]) cudaFree(sp.mig_idx[b]);
-            for (int b = 0; b < 4; ++b) if (sp.mig_msg[b]) cudaFree(sp.mig_msg[b]);
-            if (sp.mig_work) cudaFree(sp.mig_work);
-            if (sp.mig_head) cudaFreeHost(sp.mig_head);
-            if (sp.bnd_work) cudaFree(sp.bnd_work);
-            if (sp.spent_work) cudaFree(sp.spent_work);
-        }
-        for (auto& L : e->lasers) { if (L.bnd_work) cudaFree(L.bnd_work); if (L.w_owned) cudaFree(L.w_owned); }
-        if (e->shift_tmp) cudaFree(e->shift_tmp);
-        if (e->nci_alloc) for (int c = 0; c < 6; ++c) cudaFree(e->nci_fab[c].p);
-        if (e->host_count) cudaFreeHost(e->host_count);
-        if (e->coll_status) cudaFree(e->coll_status);
-        for (auto& c : e->collisions) if (c.work) cudaFree(c.work);
-        for (int b = 0; b < 4; ++b) if (e->hbuf[b]) cudaFree(e->hbuf[b]);
-    }
     delete e;
 }
 extern "C" double pic_engine_dt(void* h) { return static_cast<Engine*>(h)->dt; }
@@ -995,7 +1018,7 @@ extern "C" void pic_engine_guards(void* h, int out[12]) {
 }
 extern "C" int pic_engine_set_fields(void* h, const pic_fab fabs[9]) {
     Engine* e = static_cast<Engine*>(h);
-    if (e->jdep_alloc) { for (int c = 0; c < 3; ++c) cudaFree(e->jdep[c].p); e->jdep_alloc = false; }   // new shapes
+    for (auto& m : e->jdep_mem) m.release();     // new shapes
     for (int c = 0; c < 9; ++c) {
         e->fab[c] = fabs[c];
         const int* ng = c < 6 ? e->ng_EB : e->ng_J;
@@ -1017,27 +1040,24 @@ extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(capacity >= bufA->np, "pic_engine_add_species: capacity %ld < np %ld", capacity, (long)bufA->np);
     PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_species: runs with fluid species take no particle species yet");
-    Species sp;
+    pic_bins bins{};
+    bins.cell_start = cell_start;
+    for (int d = 0; d < 3; ++d) {
+        bins.box_lo[d] = e->box_lo[d]; bins.box_hi[d] = e->box_hi[d];
+        bins.tile[d] = tile ? tile[d] : 8;
+    }
+    // Everything is allocated for a local species; the engine takes it only when the call succeeds.
+    Species sp(q, m, bins);
     sp.capacity = capacity;
     sp.next_id = (uint64_t)bufA->np;     // ids of particles created later (fusion products) follow the initial ones
-    sp.q = q; sp.m = m; sp.buf[0] = *bufA; sp.buf[1] = *bufB; sp.cur = 0; sp.has_bins = false; sp.sort_work = sort_work;
-    sp.bins.cell_start = cell_start;
-    for (int d = 0; d < 3; ++d) sp.bins.tile[d] = tile ? tile[d] : 8;
-    sp.bins.np_binned = 0;
+    sp.buf[0] = *bufA; sp.buf[1] = *bufB; sp.sort_work = sort_work;
     // escape list: a layer of one cell next to every domain face can leave per step at most
-    sp.has_esc = false;
-    {
-        const long cap = capacity / 16 + 65536;
-        int* mem = nullptr;
-        if (cudaMalloc(&mem, sizeof(int) * (size_t)(cap + 1)) == cudaSuccess) {
-            sp.esc.count = mem; sp.esc.idx = mem + 1; sp.esc.capacity = (int)cap;
-            for (int d = 0; d < 3; ++d) {
-                sp.esc.lo[d] = e->geom.periodic[d] ? e->geom.prob_lo[d] : -INFINITY;
-                sp.esc.hi[d] = e->geom.periodic[d] ? e->geom.prob_hi[d] : INFINITY;
-            }
-            sp.has_esc = true;
-        } else {
-            cudaGetLastError();      // no list: the engine wraps with the full sweep
+    const long esc_cap = capacity / 16 + 65536;
+    if (sp.esc_mem.try_alloc(sizeof(int) * (size_t)(esc_cap + 1))) {
+        sp.esc.count = sp.esc_mem.get(); sp.esc.idx = sp.esc_mem.get() + 1; sp.esc.capacity = (int)esc_cap;
+        for (int d = 0; d < 3; ++d) {
+            sp.esc.lo[d] = e->geom.periodic[d] ? e->geom.prob_lo[d] : -INFINITY;
+            sp.esc.hi[d] = e->geom.periodic[d] ? e->geom.prob_hi[d] : INFINITY;
         }
     }
     if (e->comm) {
@@ -1050,19 +1070,21 @@ extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa
         }
         sp.mig_cap = sp.mig_cap_max;
         const size_t nmsg = (size_t)pic_migrate_message_doubles(sp.mig_cap_max);
-        bool ok = cudaMalloc(&sp.mig_counts, 2 * sizeof(int)) == cudaSuccess;
-        for (int b = 0; b < 2 && ok; ++b) ok = cudaMalloc(&sp.mig_idx[b], sizeof(int) * (size_t)sp.mig_cap_max) == cudaSuccess;
-        for (int b = 0; b < 4 && ok; ++b) ok = cudaMalloc(&sp.mig_msg[b], sizeof(double) * nmsg) == cudaSuccess;
-        ok = ok && cudaMalloc(&sp.mig_work, (size_t)pic_migrate_workspace_bytes(sp.mig_cap_max)) == cudaSuccess;
-        ok = ok && cudaMallocHost(&sp.mig_head, 8 * sizeof(int)) == cudaSuccess;
-        if (!ok) return fail("pic_engine_add_species: cannot allocate the migration buffers");
-        for (int b = 0; b < 4; ++b) cudaMemsetAsync(sp.mig_msg[b], 0, sizeof(double) * nmsg, (cudaStream_t)stream);
-        cudaMemsetAsync(sp.mig_work, 0, (size_t)pic_migrate_workspace_bytes(sp.mig_cap_max), (cudaStream_t)stream);
+        const char* what = "pic_engine_add_species: cannot allocate the migration buffers";
+        ENG_CALL(sp.mig_counts.alloc(2 * sizeof(int), what));
+        for (auto& b : sp.mig_idx) ENG_CALL(b.alloc(sizeof(int) * (size_t)sp.mig_cap_max, what));
+        for (auto& b : sp.mig_msg) ENG_CALL(b.alloc(sizeof(double) * nmsg, what));
+        ENG_CALL(sp.mig_work.alloc((size_t)pic_migrate_workspace_bytes(sp.mig_cap_max), what));
+        ENG_CALL(sp.mig_head.alloc(8 * sizeof(int), what));
+        for (auto& b : sp.mig_msg) cudaMemsetAsync(b.get(), 0, sizeof(double) * nmsg, (cudaStream_t)stream);
+        cudaMemsetAsync(sp.mig_work.get(), 0, (size_t)pic_migrate_workspace_bytes(sp.mig_cap_max), (cudaStream_t)stream);
     }
-    if (!e->all_periodic) ENG_CALL(alloc_boundary_scratch(capacity, &sp.bnd_work, &sp.bnd_cap));
-    e->species.push_back(sp);
-    ENG_CALL(grow_host_counts(*e));
-    if (cell_start && sort_work) return sort_species(*e, e->species.back(), false, stream);
+    if (!e->all_periodic) ENG_CALL(alloc_boundary_scratch(capacity, sp.bnd_work, &sp.bnd_cap));
+    PinnedBuf<int> counts;
+    ENG_CALL(alloc_host_counts_for_one_more(*e, counts));
+    if (cell_start && sort_work) ENG_CALL(sort_species(*e, sp, false, stream));
+    e->species.push_back(std::move(sp));
+    e->host_count = std::move(counts);
     return 0;
 }
 // Multi-rank: this rank's brick is box_lo..box_hi of pic_engine_create, rank = coord[0] + nb[0]*(coord[1]
@@ -1133,29 +1155,14 @@ extern "C" int pic_engine_redistribute(void* h, void* stream) {
     for (auto& L : e->lasers) ENG_CALL(pic_particles_wrap_periodic(&L.P, &e->geom, stream));
     ENG_CALL(apply_particle_boundaries(*e, stream));
     for (auto& sp : e->species) {
-        sp.esc_valid = false;            // the caller moved the particles, not the push: classify every one
+        sp.ord.escape_list_spent();      // the caller moved the particles, not the push: classify every one
         if (e->comm) ENG_CALL(migrate(*e, sp, stream));
-        sp.bins_stale = true;
+        sp.ord.cells_changed();
     }
     return 0;
 }
 
 // ---- non-periodic runs ------------------------------------------------------------------------
-static int alloc_boundary_scratch(long capacity, int** work, int* cap) {
-    const long c = capacity / 16 + 65536;
-    *cap = (int)(c < capacity + 1 ? c : capacity + 1);
-    if (cudaMalloc(work, sizeof(int) * (size_t)pic_particles_boundary_workspace_ints(*cap)) != cudaSuccess)
-        return fail("pic_engine: cannot allocate the particle-boundary scratch");
-    return 0;
-}
-static int grow_host_counts(Engine& e) {
-    const size_t n = e.species.size() + e.lasers.size() + 1;
-    int* mem = nullptr;
-    if (cudaMallocHost(&mem, sizeof(int) * n) != cudaSuccess) return fail("pic_engine: cannot allocate pinned host memory");
-    if (e.host_count) cudaFreeHost(e.host_count);
-    e.host_count = mem;
-    return 0;
-}
 extern "C" int pic_engine_set_boundaries(void* h, const pic_boundaries* b) {
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(e->species.empty() && e->lasers.empty(), "pic_engine_set_boundaries: call before adding particles");
@@ -1238,11 +1245,14 @@ extern "C" int pic_engine_add_laser(void* h, const pic_laser_antenna* prm, const
     PIC_REQUIRE(capacity >= p->np, "pic_engine_add_laser: capacity %ld < np %ld", capacity, (long)p->np);
     Laser L;
     L.prm = *prm; L.P = *p; L.capacity = capacity;
-    if (!e->all_periodic) ENG_CALL(alloc_boundary_scratch(capacity, &L.bnd_work, &L.bnd_cap));
-    if (e->comm && cudaMalloc(&L.w_owned, sizeof(double) * (size_t)(capacity > 0 ? capacity : 1)) != cudaSuccess)
-        return fail("pic_engine_add_laser: cannot allocate the weight scratch");
-    e->lasers.push_back(L);
-    return grow_host_counts(*e);
+    if (!e->all_periodic) ENG_CALL(alloc_boundary_scratch(capacity, L.bnd_work, &L.bnd_cap));
+    if (e->comm) ENG_CALL(L.w_owned.alloc(sizeof(double) * (size_t)(capacity > 0 ? capacity : 1),
+                                          "pic_engine_add_laser: cannot allocate the weight scratch"));
+    PinnedBuf<int> counts;
+    ENG_CALL(alloc_host_counts_for_one_more(*e, counts));
+    e->lasers.push_back(std::move(L));
+    e->host_count = std::move(counts);
+    return 0;
 }
 extern "C" long pic_engine_laser_np(void* h, int il) { return (long)static_cast<Engine*>(h)->lasers[il].P.np; }
 extern "C" double pic_engine_time(void* h) { return static_cast<Engine*>(h)->cur_time; }
@@ -1266,14 +1276,14 @@ extern "C" int pic_engine_species_buffer(void* h, int isp, long* np) {
 // WarpX::Evolve(numsteps): the last step synchronises u with x when synchronize_last is set
 extern "C" int pic_engine_evolve(void* h, int numsteps, int synchronize_last, void* stream) {
     Engine* e = static_cast<Engine*>(h);
-    if (!e->collisions.empty()) cudaMemsetAsync(e->coll_status, 0, sizeof(int), (cudaStream_t)stream);
+    if (!e->collisions.empty()) cudaMemsetAsync(e->coll_status.get(), 0, sizeof(int), (cudaStream_t)stream);
     for (int n = 0; n < numsteps; ++n) {
         const bool final_step = n == numsteps - 1;
         ENG_CALL(one_step(*e, synchronize_last && final_step, !final_step, stream));
     }
     if (!e->collisions.empty()) {        // one read per call: did a cell exceed the collision kernel's capacity?
         int st = 0;
-        cudaMemcpyAsync(&st, e->coll_status, sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
+        cudaMemcpyAsync(&st, e->coll_status.get(), sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
         if (cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
             return fail("pic_engine_evolve: %s", cudaGetErrorString(cudaGetLastError()));
         PIC_REQUIRE(st == 0, "pic_engine_evolve: a collision found no scratch for a cell of more than 2048 particles");
@@ -1281,34 +1291,36 @@ extern "C" int pic_engine_evolve(void* h, int numsteps, int synchronize_last, vo
     return 0;
 }
 
+// The refusals every collision entry shares (who: the calling function); checked before the engine changes.
+static int check_collision_entry(const Engine& e, const char* who, int isp1, int isp2, int ndt) {
+    const int nsp = (int)e.species.size();
+    PIC_REQUIRE(isp1 >= 0 && isp1 < nsp && isp2 >= 0 && isp2 < nsp, "%s: no species %d / %d", who, isp1, isp2);
+    PIC_REQUIRE(ndt >= 1, "%s: ndt must be at least 1 (got %d)", who, ndt);
+    PIC_REQUIRE(e.fluids.empty(), "%s: runs with fluid species take no collisions", who);
+    PIC_REQUIRE(e.comm == nullptr, "%s: one rank only (collisions over several ranks are not yet checked against a "
+                                   "single box)", who);
+    for (int isp : {isp1, isp2}) {
+        const pic_bins& b = e.species[isp].ord.bins();
+        PIC_REQUIRE(e.species[isp].sort_work && b.cell_start, "%s: species %d has no cell bins", who, isp);
+        for (int d = 0; d < 3; ++d)
+            PIC_REQUIRE(b.tile[d] == e.species[isp1].ord.bins().tile[d], "%s: the species' bins use different tiles", who);
+    }
+    return 0;
+}
+
 extern "C" int pic_engine_add_collision(void* h, int isp1, int isp2, double coulomb_log, int ndt, uint64_t seed) {
     Engine* e = static_cast<Engine*>(h);
     PIC_REQUIRE(e, "pic_engine_add_collision: no engine");
-    const int nsp = (int)e->species.size();
-    PIC_REQUIRE(isp1 >= 0 && isp1 < nsp && isp2 >= 0 && isp2 < nsp, "pic_engine_add_collision: no species %d / %d", isp1, isp2);
-    PIC_REQUIRE(ndt >= 1, "pic_engine_add_collision: ndt must be at least 1 (got %d)", ndt);
-    PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_collision: runs with fluid species take no collisions");
-    PIC_REQUIRE(e->comm == nullptr, "pic_engine_add_collision: one rank only (collisions over several ranks are not "
-                                    "yet checked against a single box)");
-    for (int isp : {isp1, isp2}) {
-        const Species& sp = e->species[isp];
-        PIC_REQUIRE(sp.sort_work && sp.bins.cell_start, "pic_engine_add_collision: species %d has no cell bins", isp);
-        for (int d = 0; d < 3; ++d)
-            PIC_REQUIRE(sp.bins.tile[d] == e->species[isp1].bins.tile[d], "pic_engine_add_collision: the species' bins use different tiles");
-    }
-    if (!e->coll_status) {
-        if (cudaMalloc(&e->coll_status, sizeof(int)) != cudaSuccess) {
-            cudaGetLastError();
-            e->coll_status = nullptr;
-            return fail("pic_engine_add_collision: cannot allocate the status word");
-        }
-    }
+    ENG_CALL(check_collision_entry(*e, "pic_engine_add_collision", isp1, isp2, ndt));
     // a Coulomb entry after a fusion on one of its species would meet the reactants that fusion spent in the same step
     // (they leave at the end of the step); the reference removes them between the two collisions
     for (const Collision& c : e->collisions)
         PIC_REQUIRE(!c.fusion || (c.isp1 != isp1 && c.isp1 != isp2 && c.isp2 != isp1 && c.isp2 != isp2),
                     "pic_engine_add_collision: species %d / %d are reactants of an earlier fusion entry; register the "
                     "Coulomb collision before the fusion", isp1, isp2);
+    DeviceBuf<int> status;
+    if (!e->coll_status) ENG_CALL(status.alloc(sizeof(int), "pic_engine_add_collision: cannot allocate the status word"));
+    if (status) e->coll_status = std::move(status);
     e->collisions.push_back(Collision{isp1, isp2, ndt, coulomb_log, seed});
     return 0;
 }
@@ -1368,42 +1380,29 @@ extern "C" int pic_engine_add_fusion(void* h, int isp1, int isp2, int iprodA, in
         PIC_REQUIRE(i != isp1 && i != isp2, "pic_engine_add_fusion: a product species (%d) cannot be a reactant", i);
     PIC_REQUIRE(multiplier > 0.0 && probability_threshold > 0.0 && probability_target_value > 0.0,
                 "pic_engine_add_fusion: the multiplier, threshold and target value must be positive");
-    PIC_REQUIRE(ndt >= 1, "pic_engine_add_fusion: ndt must be at least 1 (got %d)", ndt);
-    PIC_REQUIRE(e->fluids.empty(), "pic_engine_add_fusion: runs with fluid species take no collisions");
-    PIC_REQUIRE(e->comm == nullptr, "pic_engine_add_fusion: one rank only (collisions over several ranks are not "
-                                    "yet checked against a single box)");
-    for (int isp : {isp1, isp2}) {
-        const Species& sp = e->species[isp];
-        PIC_REQUIRE(sp.sort_work && sp.bins.cell_start, "pic_engine_add_fusion: species %d has no cell bins", isp);
-        for (int d = 0; d < 3; ++d)
-            PIC_REQUIRE(sp.bins.tile[d] == e->species[isp1].bins.tile[d], "pic_engine_add_fusion: the species' bins use different tiles");
-    }
+    ENG_CALL(check_collision_entry(*e, "pic_engine_add_fusion", isp1, isp2, ndt));
     Collision c{isp1, isp2, ndt, 0.0, seed};
     c.fusion = true; c.iprod[0] = iprodA; c.iprod[1] = iprodB; c.type = type;
     c.multiplier = multiplier; c.threshold = probability_threshold; c.target = probability_target_value;
     c.pair_cap = e->species[isp1].capacity + (isp1 == isp2 ? 0 : e->species[isp2].capacity);
-    const long nbins = pic_bins_count(e->box_lo, e->box_hi, e->species[isp1].bins.tile);
-    bool ok = cudaMalloc(&c.work, (size_t)pic_fusion_workspace_bytes(c.pair_cap, nbins)) == cudaSuccess;
-    if (ok && !e->coll_status) ok = cudaMalloc(&e->coll_status, sizeof(int)) == cudaSuccess;
-    int* spent[2] = {nullptr, nullptr};
-    for (int k = 0; k < 2 && ok; ++k) {
+    const long nbins = pic_bins_count(e->box_lo, e->box_hi, e->species[isp1].ord.bins().tile);
+    const char* what = "pic_engine_add_fusion: cannot allocate the fusion workspace";
+    ENG_CALL(c.work.alloc((size_t)pic_fusion_workspace_bytes(c.pair_cap, nbins), what));
+    DeviceBuf<int> status, spent[2];
+    if (!e->coll_status) ENG_CALL(status.alloc(sizeof(int), what));
+    for (int k = 0; k < 2; ++k) {
         const Species& sp = e->species[k ? isp2 : isp1];
         if (sp.spent_work || (k == 1 && isp1 == isp2)) continue;
-        ok = cudaMalloc(&spent[k], sizeof(int) * (size_t)pic_particles_boundary_workspace_ints((int)(sp.capacity + 1))) == cudaSuccess;
+        ENG_CALL(spent[k].alloc(sizeof(int) * (size_t)pic_particles_boundary_workspace_ints((int)(sp.capacity + 1)), what));
     }
-    if (!ok) {
-        cudaGetLastError();
-        if (c.work) cudaFree(c.work);
-        for (int* p : spent) if (p) cudaFree(p);
-        return fail("pic_engine_add_fusion: cannot allocate the fusion workspace");
-    }
+    if (status) e->coll_status = std::move(status);
     for (int k = 0; k < 2; ++k)
         if (spent[k]) {
             Species& sp = e->species[k ? isp2 : isp1];
-            sp.spent_work = spent[k];
+            sp.spent_work = std::move(spent[k]);
             sp.spent_cap = (int)(sp.capacity + 1);
         }
-    e->collisions.push_back(c);
+    e->collisions.push_back(std::move(c));
     return 0;
 }
 

@@ -54,7 +54,12 @@ static GatherGeom make_gather_geom(const pic_fab E[3], const pic_fab B[3], const
 }
 }
 
-namespace pic { extern int g_gather_mode; }      // gather_push_tile.cu
+namespace pic {
+extern int g_gather_mode;      // gather_push_tile.cu
+// Whether pic_gather_push_permuted serves shape order nox: only the default supercell kernel, built for orders 1..3,
+// carries out a pending cell sort.
+bool gather_push_carries_permutation(int nox) { return nox >= 1 && nox <= 3 && g_gather_mode == PIC_GATHER_TILE; }
+}
 extern "C" void pic_set_gather_mode(int mode) { pic::g_gather_mode = (mode >= PIC_GATHER_PAIRS && mode <= PIC_GATHER_PAIRS_192) ? mode : 0; }
 
 extern "C" int pic_gather_push(const pic_soa* p, long offset, long np, const pic_fab E[3],
@@ -113,7 +118,7 @@ extern "C" int pic_gather_push_permuted(const pic_soa* in, const pic_soa* out, c
     PIC_REQUIRE(nox >= 1 && nox <= 3, "pic_gather_push_permuted: the supercell kernel serves orders 1..3, not %d", nox);
     PIC_REQUIRE(galerkin == 0 || galerkin == 1, "pic_gather_push_permuted: galerkin must be 0/1");
     PIC_REQUIRE(pusher >= 0 && pusher <= 2, "pic_gather_push_permuted: unknown particle pusher %d", pusher);
-    PIC_REQUIRE(pic::g_gather_mode == PIC_GATHER_TILE, "pic_gather_push_permuted: only the default gather kernel permutes (gather mode %d is set)", pic::g_gather_mode);
+    PIC_REQUIRE(pic::gather_push_carries_permutation(nox), "pic_gather_push_permuted: only the default gather kernel permutes (gather mode %d is set)", pic::g_gather_mode);
     if (in->np == 0) return 0;
     PermSrc perm;
     perm.in = make_soa(*in, 0); perm.src = src; perm.id_in = in->idcpu; perm.id_out = out->idcpu;
