@@ -11,7 +11,7 @@ sorts ndt = 1 forces), the whole step with and without collisions, and the achie
 stage's algorithmic bytes -- per particle: read id, w, ux, uy, uz and src, write ux, uy, uz (68 B); per bin and species:
 one cell_start entry (4 B).  The card's name, power limit and maximum SM clock are read in the same run.
 The fp64 instruction count is the static count of double-precision instructions in the SASS of the collision kernels
-(cuobjdump of the library).
+(cuobjdump of the library): the cell walk's kernels instantiated with PairwiseCoulomb.
 
     python tools/bench_collisions.py --steps 10 --warmup 3 > bench_collisions.json"""
 import argparse
@@ -41,7 +41,7 @@ def sass_fp64_counts():
     for line in sass.splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
-            cur = m.group(1) if "coll" in m.group(1) and "collide" in m.group(1) else None
+            cur = m.group(1) if "kernel" in m.group(1) and "PairwiseCoulomb" in m.group(1) else None
             if cur:
                 out[cur] = {"fp64": 0, "all": 0}
             continue

@@ -2,8 +2,9 @@
 // proton-boron.
 //
 // Restates, for one tile = the rank's box (paths relative to Source/Particles/Collision/BinaryCollision/):
-//   fuse_cell / chains   <- BinaryCollision::doCollisionsWithinTile  BinaryCollision.H:383-472 (intra-species, halves),
-//                           :613-730 (inter-species), with NuclearFusionFunc::Executor  NuclearFusion/NuclearFusionFunc.H:127-234
+//   the cell walk        <- BinaryCollision::doCollisionsWithinTile  BinaryCollision.H:383-472 (intra-species, halves),
+//   (binary_collision.cuh)  :613-730 (inter-species)
+//   NuclearFusion        <- NuclearFusionFunc::Executor                                NuclearFusion/NuclearFusionFunc.H:127-234
 //   collision_parameters <- BinaryCollisionUtils::get_collision_parameters             BinaryCollisionUtils.H
 //   bosch_hale           <- BoschHaleFusionCrossSection                                NuclearFusion/BoschHaleFusionCrossSection.H
 //   fusion_event         <- SingleNuclearFusionEvent                                   NuclearFusion/SingleNuclearFusionEvent.H
@@ -30,10 +31,9 @@
 //     writes slots 2e, 2e + 1 of each product, a proton-boron event slots 6e + 2k, 6e + 2k + 1 of alpha k = 0, 1, 2;
 //   * the file is compiled without FMA contraction.
 //
-// Event pass: one pass over the bins with the Coulomb pass's grouping -- a warp per cell of at most SMALL_CAP
-// particles, a 256-thread block per cell of at most LARGE_CAP, and beyond that a block that keeps only the cell's
-// canonical order in the caller's per-slot scratch.  A cell's pairs go to records at its own slots (cell_start of
-// species 1 plus that of species 2), its pair and event counts to per-bin arrays: no global atomics.  Product pass:
+// Event pass: one pass of the cell walk of binary_collision.cuh over the bins, the Coulomb pass's walk, leaving spent
+// particles out.  A cell's pairs go to records at its own slots (cell_start of species 1 plus that of species 2), its
+// pair and event counts to per-bin arrays: no global atomics.  Product pass:
 // an exclusive scan of the event counts, one host read of the total, a warp per bin writing its events' products in
 // pair order.
 #include "binary_collision.cuh"
@@ -47,21 +47,14 @@ using coll::Stream;
 using coll::dmax;
 using coll::dmin;
 using coll::DBL_MIN_;
+using coll::HBAR;
 using coll::PI;
 
 constexpr double Q_E = 1.602176634e-19;         // PhysConst::q_e
 constexpr double ALPHA = 0.007297352573748943;  // PhysConst::alpha
 constexpr double M_U = 1.66053906660e-27;      // PhysConst::m_u
-constexpr double EP0 = 8.8541878128e-12;       // PhysConst::ep0
-constexpr double HBAR = 1.054571817e-34;       // PhysConst::hbar
 constexpr double C_SQ = C_LIGHT * C_LIGHT;
 constexpr double INV_CSQ = 1.0 / C_SQ;
-
-constexpr int SMALL_CAP = 64;
-constexpr int SMALL_WARPS = 4;
-constexpr int LARGE_CAP = 2048;
-constexpr int LARGE_THREADS = 256;
-constexpr int LARGE_SCAN = 32;
 constexpr uint64_t PRODUCT_TAG = 1ull << 62;
 
 static size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
@@ -101,22 +94,6 @@ static Work carve(void* base, long pc, long nbins, size_t* total = nullptr) {
     if (total) *total = off;
     return w;
 }
-
-struct Args {
-    SoaView P1, P2;
-    uint64_t* id1; uint64_t* id2;
-    const int* src1; const int* src2;
-    int* scr1; int* scr2;
-    BinsView b1, b2;
-    int gn[2];
-    double m1, m2, dt, dV;
-    double mult, thr, target;
-    int type;
-    uint64_t seed, cidx, step;
-    int same;
-    Work wk;
-    int* status;
-};
 
 // BinaryCollisionUtils::get_collision_parameters: kinetic energy and relative velocity in the centre-of-momentum frame,
 // and the ratio of its Lorentz factors to the lab frame's
@@ -326,263 +303,62 @@ __host__ __device__ __forceinline__ void alpha_momenta(double u1x, double u1y, d
     u[2][0] = (px_Be - px2) / m_alpha; u[2][1] = (py_Be - py2) / m_alpha; u[2][2] = (pz_Be - pz2) / m_alpha;
 }
 
-// first record slot of the bin's pairs: [cs1 + cs2, + n1 + n2) of one bin never overlaps another's
-__device__ __forceinline__ long pair_base(const Args& a, long bin) {
-    return a.b1.cell_start[bin] + (a.same ? 0 : a.b2.cell_start[bin]);
-}
+// The cell walk's functor (binary_collision.cuh) for NuclearFusionFunc::Executor: pair k of a cell goes to the record
+// base + k of the workspace, a reactant that an event leaves with w <= DBL_MIN is spent.
+struct NuclearFusion {
+    struct Args : coll::PairArgs {
+        double mult, thr, target;
+        int type;
+        Work wk;
+    };
+    static constexpr bool skip_spent = true;
+    struct Scalars { int live[2], events; };   // live particles of each species, events of the cell
 
-// particles of the cell's species 1 (and 2), spent ones included; 0 when fewer than a pair's worth are stored
-__device__ __forceinline__ int cell_load(const Args& a, long bin, long* cs1, int* n1, long* cs2, int* n2) {
-    *cs1 = a.b1.cell_start[bin];
-    *n1 = a.b1.cell_start[bin + 1] - (int)*cs1;
-    if (a.same) { *cs2 = *cs1; *n2 = 0; return *n1 >= 2 ? *n1 : 0; }
-    *cs2 = a.b2.cell_start[bin];
-    *n2 = a.b2.cell_start[bin + 1] - (int)*cs2;
-    return (*n1 >= 1 && *n2 >= 1) ? *n1 + *n2 : 0;
-}
+    template <class V> __device__ static void species(const Args&, const V&, int, const int*, int, Scalars&) {}
 
-__device__ __forceinline__ void shuffle(const Args& a, int* sh, int n, uint64_t gcell, int tag) {
-    Stream rng(a.seed, a.step, gcell, (a.cidx << 32) | (uint64_t)tag);
-    for (int i = n - 1; i >= 1; --i) {
-        const int j = rng.random_int(i + 1);
-        const int t = sh[i]; sh[i] = sh[j]; sh[j] = t;
-    }
-}
+    long base;                 // first record of the cell: [cs1 + cs2, + n1 + n2) of one bin never overlaps another's
+    int multiplier_ratio, npairs, events;
 
-// The pair chains of one cell (NuclearFusionFunc::Executor), chain c by thread c, c + G, ...: pairs (I1[i1], I2[i2])
-// of the index sets into w1 / w2 and u1 / u2, whose spent flags are dead1 / dead2 (entries of the same arrays for an
-// intra-species collision); pos1 / pos2 give a particle's storage index.  Pair k of the cell goes to record base + k.
-// Returns this thread's number of events.
-template <int G>
-__device__ int chains(const Args& a, int t, uint64_t gcell, long base, const int* I1, const int* I2, int NI1, int NI2,
-                      double* w1, const double* u1x, const double* u1y, const double* u1z, unsigned char* dead1,
-                      const int* pos1, double* w2, const double* u2x, const double* u2y, const double* u2z,
-                      unsigned char* dead2, const int* pos2) {
-    const int maxN = NI1 > NI2 ? NI1 : NI2, minN = NI1 < NI2 ? NI1 : NI2;
-    const int multiplier_ratio = a.same ? minN + maxN - 1 : minN;
-    const double m2 = a.same ? a.m1 : a.m2;
-    int events = 0;
-    for (int c = t; c < minN; c += G) {
-        Stream rng(a.seed, a.step, gcell, (a.cidx << 32) | (uint64_t)(2 + c));
-        int i1 = c, i2 = c;
-        for (int k = c; k < maxN; k += minN) {
-            const int e1 = I1[i1], e2 = I2[i2];
-            bool ev = false;
-            double wr = 0.0;
-            if (!dead1[e1] && !dead2[e2]) {
-                ev = fusion_event(u1x[e1], u1y[e1], u1z[e1], u2x[e2], u2y[e2], u2z[e2], a.m1, m2, w1[e1], w2[e2], a.dt,
-                                  a.dV, a.mult, multiplier_ratio, a.thr, a.target, a.type, rng, &wr);
-                if (ev) {                      // BinaryCollisionUtils::remove_weight_from_colliding_particle
-                    w1[e1] = w1[e1] + -wr;
-                    if (w1[e1] <= DBL_MIN_) dead1[e1] = 1;
-                    w2[e2] = w2[e2] + -wr;
-                    if (w2[e2] <= DBL_MIN_) dead2[e2] = 1;
-                    ++events;
-                }
+    __device__ NuclearFusion(const Args& a, long bin, const Scalars&, int minN, int maxN)
+        : base(a.b1.cell_start[bin] + (a.same ? 0 : a.b2.cell_start[bin])),
+          multiplier_ratio(a.same ? minN + maxN - 1 : minN), npairs(maxN), events(0) {}
+
+    // pairs with a spent reactant draw nothing (NuclearFusionFunc.H:181-184)
+    template <class V>
+    __device__ void pair(const Args& a, const V& v, int e1, int e2, int k, Stream& rng) {
+        bool ev = false;
+        double wr = 0.0;
+        if (!v.spent(1, e1) && !v.spent(2, e2)) {
+            ev = fusion_event(v.ux(1, e1), v.uy(1, e1), v.uz(1, e1), v.ux(2, e2), v.uy(2, e2), v.uz(2, e2), a.m1,
+                              a.same ? a.m1 : a.m2, v.w(1, e1), v.w(2, e2), a.dt, a.dV, a.mult, multiplier_ratio, a.thr,
+                              a.target, a.type, rng, &wr);
+            if (ev) {                          // BinaryCollisionUtils::remove_weight_from_colliding_particle
+                v.w(1, e1) = v.w(1, e1) + -wr;
+                if (v.w(1, e1) <= DBL_MIN_) v.spend(1, e1);
+                v.w(2, e2) = v.w(2, e2) + -wr;
+                if (v.w(2, e2) <= DBL_MIN_) v.spend(2, e2);
+                ++events;
             }
-            const long r = base + k;
-            a.wk.slot1[r] = pos1[e1]; a.wk.slot2[r] = pos2[e2];
-            a.wk.wr[r] = wr; a.wk.mask[r] = ev ? 1 : 0;
-            if (maxN == NI1) i1 += minN;
-            if (maxN == NI2) i2 += minN;
         }
+        const long r = base + k;
+        a.wk.slot1[r] = v.storage(1, e1); a.wk.slot2[r] = v.storage(2, e2);
+        a.wk.wr[r] = wr; a.wk.mask[r] = ev ? 1 : 0;
     }
-    return events;
-}
 
-// Shared memory of one group for `cap` particles: w ux uy uz (canonical order), ids (load order), storage index (load
-// order), storage index (canonical order), shuffled positions, spent flags (canonical order), 2 counters.
-__host__ __device__ constexpr size_t group_bytes(int cap) { return (size_t)cap * (4 * 8 + 8 + 3 * 4 + 1) + 16; }
+    template <int G> __device__ void end_cell(const Args& a, long bin, int t, Scalars& x) const {
+        if (events) atomicAdd(&x.events, events);   // shared memory only
+        coll::group_sync<G>();
+        if (t == 0) { a.wk.npairs[bin] = npairs; a.wk.events[bin] = x.events; }
+    }
 
-struct Group {
-    double *w, *ux, *uy, *uz;
-    uint64_t* key;
-    int *lp, *pp, *sh, *cnt;
-    unsigned char* dead;
-    __device__ Group(char* base, int cap) {
-        double* d = reinterpret_cast<double*>(base);
-        w = d; ux = d + cap; uy = d + 2 * cap; uz = d + 3 * cap;
-        key = reinterpret_cast<uint64_t*>(d + 4 * cap);
-        lp = reinterpret_cast<int*>(key + cap); pp = lp + cap; sh = pp + cap; cnt = sh + cap;
-        dead = reinterpret_cast<unsigned char*>(cnt + 4);
+    template <class V>
+    __device__ static void store(const Args& a, const V& v, int sp, int e) {
+        const SoaView& P = sp == 1 ? a.P1 : a.P2;
+        const int p = v.storage(sp, e);
+        P.w[p] = v.w(sp, e);
+        if (v.spent(sp, e)) (sp == 1 ? a.id1 : a.id2)[p] = PIC_SPENT_ID;
     }
 };
-
-// One cell with n = n1 + n2 stored particles (n1 for intra-species), 0 < n <= cap, by a group of G threads.
-template <int G>
-__device__ void fuse_cell(const Args& a, long bin, int t, char* smem, int cap, long cs1, int n1, long cs2, int n2) {
-    Group s(smem, cap);
-    const int n = n1 + n2;
-    if (t == 0) { s.cnt[0] = 0; s.cnt[1] = 0; s.cnt[2] = 0; }
-    for (int e = t; e < n; e += G) {
-        const int p = coll::storage_index(a, e, n1, cs1, cs2);
-        s.key[e] = (e >= n1 ? a.id2 : a.id1)[p];
-        s.lp[e] = p;
-    }
-    coll::group_sync<G>();
-    // canonical order of the live particles: rank by id inside each species; spent ids (the largest value) rank last
-    for (int e = t; e < n; e += G) {
-        const bool two = e >= n1;
-        const int lo = two ? n1 : 0, hi = two ? n : n1;
-        const uint64_t k = s.key[e];
-        if (k == PIC_SPENT_ID) continue;
-        atomicAdd(&s.cnt[two ? 1 : 0], 1);                     // shared memory only
-        int r = lo;
-        for (int f = lo; f < hi; ++f) { const uint64_t kf = s.key[f]; r += (kf < k) || (kf == k && f < e); }
-        const int p = s.lp[e];
-        const SoaView& P = two ? a.P2 : a.P1;
-        s.pp[r] = p;
-        s.w[r] = P.w[p]; s.ux[r] = P.ux[p]; s.uy[r] = P.uy[p]; s.uz[r] = P.uz[p];
-        s.dead[r] = 0;
-        s.sh[r] = r;
-    }
-    coll::group_sync<G>();
-    const int L1 = s.cnt[0], L2 = s.cnt[1];
-    coll::group_sync<G>();                                     // read by all before the next cell resets them
-    if (a.same ? L1 < 2 : (L1 < 1 || L2 < 1)) return;          // uniform over the group
-    const uint64_t gcell = coll::global_cell(a, bin);
-    constexpr int second = G == 32 ? 1 : 32;
-    if (t == 0) shuffle(a, s.sh, L1, gcell, 0);
-    if (t == second && !a.same) shuffle(a, s.sh + n1, L2, gcell, 1);
-    coll::group_sync<G>();
-    const int half = L1 / 2;
-    const int NI1 = a.same ? half : L1, NI2 = a.same ? L1 - half : L2;
-    const int ev = chains<G>(a, t, gcell, pair_base(a, bin), s.sh, a.same ? s.sh + half : s.sh + n1, NI1, NI2, s.w, s.ux,
-                             s.uy, s.uz, s.dead, s.pp, s.w, s.ux, s.uy, s.uz, s.dead, s.pp);
-    if (ev) atomicAdd(&s.cnt[2], ev);
-    coll::group_sync<G>();
-    if (t == 0) { a.wk.npairs[bin] = NI1 > NI2 ? NI1 : NI2; a.wk.events[bin] = s.cnt[2]; }
-    const int nl = a.same ? L1 : n1 + L2;
-    for (int e = t; e < nl; e += G) {
-        if (e >= L1 && e < n1) continue;
-        const bool two = e >= n1;
-        const SoaView& P = two ? a.P2 : a.P1;
-        const int p = s.pp[e];
-        P.w[p] = s.w[e];
-        if (s.dead[e]) (two ? a.id2 : a.id1)[p] = PIC_SPENT_ID;
-    }
-    coll::group_sync<G>();
-}
-
-// A cell beyond LARGE_CAP by a block on the particles in place: the canonical order of each species' live particles
-// goes to the caller's scratch at the cell's own slots; a reactant is spent when its id says so.
-__device__ void fuse_cell_global(const Args& a, long bin, int t, int* cnt, long cs1, int n1, long cs2, int n2) {
-    constexpr int G = LARGE_THREADS;
-    const int n = n1 + n2;
-    int* I1 = a.scr1 + cs1;
-    int* I2 = a.same ? nullptr : a.scr2 + cs2;
-    if (t == 0) { cnt[0] = 0; cnt[1] = 0; cnt[2] = 0; }
-    __syncthreads();
-    for (int e = t; e < n; e += G) {
-        const bool two = e >= n1;
-        const int lo = two ? n1 : 0, hi = two ? n : n1;
-        const uint64_t* id = two ? a.id2 : a.id1;
-        const int p = coll::storage_index(a, e, n1, cs1, cs2);
-        const uint64_t k = id[p];
-        if (k == PIC_SPENT_ID) continue;
-        atomicAdd(&cnt[two ? 1 : 0], 1);
-        int r = 0;
-        for (int f = lo; f < hi; ++f) {
-            const uint64_t kf = id[coll::storage_index(a, f, n1, cs1, cs2)];
-            r += (kf < k) || (kf == k && f < e);
-        }
-        (two ? I2 : I1)[r] = p;
-    }
-    __syncthreads();
-    const int L1 = cnt[0], L2 = cnt[1];
-    __syncthreads();
-    if (a.same ? L1 < 2 : (L1 < 1 || L2 < 1)) return;
-    const uint64_t gcell = coll::global_cell(a, bin);
-    if (t == 0) shuffle(a, I1, L1, gcell, 0);
-    if (t == 32 && !a.same) shuffle(a, I2, L2, gcell, 1);
-    __syncthreads();
-    const int half = L1 / 2;
-    const int NI1 = a.same ? half : L1, NI2 = a.same ? L1 - half : L2;
-    // storage indices index the particle arrays directly; "spent" is the particle's id.  The ids are written only
-    // through the spent flag below, one particle per pair chain, so no chain reads an id another one writes.
-    const int ev = [&] {
-        const int maxN = NI1 > NI2 ? NI1 : NI2, minN = NI1 < NI2 ? NI1 : NI2;
-        const int multiplier_ratio = a.same ? minN + maxN - 1 : minN;
-        const double m2 = a.same ? a.m1 : a.m2;
-        const SoaView& Q = a.same ? a.P1 : a.P2;
-        uint64_t* id2 = a.same ? a.id1 : a.id2;
-        const int* J1 = I1;
-        const int* J2 = a.same ? I1 + half : I2;
-        const long base = pair_base(a, bin);
-        int events = 0;
-        for (int c = t; c < minN; c += G) {
-            Stream rng(a.seed, a.step, gcell, (a.cidx << 32) | (uint64_t)(2 + c));
-            int i1 = c, i2 = c;
-            for (int k = c; k < maxN; k += minN) {
-                const int p1 = J1[i1], p2 = J2[i2];
-                bool evk = false;
-                double wr = 0.0;
-                if (a.id1[p1] != PIC_SPENT_ID && id2[p2] != PIC_SPENT_ID) {
-                    evk = fusion_event(a.P1.ux[p1], a.P1.uy[p1], a.P1.uz[p1], Q.ux[p2], Q.uy[p2], Q.uz[p2], a.m1, m2,
-                                       a.P1.w[p1], Q.w[p2], a.dt, a.dV, a.mult, multiplier_ratio, a.thr, a.target,
-                                       a.type, rng, &wr);
-                    if (evk) {
-                        a.P1.w[p1] = a.P1.w[p1] + -wr;
-                        if (a.P1.w[p1] <= DBL_MIN_) a.id1[p1] = PIC_SPENT_ID;
-                        Q.w[p2] = Q.w[p2] + -wr;
-                        if (Q.w[p2] <= DBL_MIN_) id2[p2] = PIC_SPENT_ID;
-                        ++events;
-                    }
-                }
-                const long r = base + k;
-                a.wk.slot1[r] = p1; a.wk.slot2[r] = p2;
-                a.wk.wr[r] = wr; a.wk.mask[r] = evk ? 1 : 0;
-                if (maxN == NI1) i1 += minN;
-                if (maxN == NI2) i2 += minN;
-            }
-        }
-        return events;
-    }();
-    if (ev) atomicAdd(&cnt[2], ev);
-    __syncthreads();
-    if (t == 0) { a.wk.npairs[bin] = NI1 > NI2 ? NI1 : NI2; a.wk.events[bin] = cnt[2]; }
-    __syncthreads();
-}
-
-__global__ void __launch_bounds__(SMALL_WARPS * 32) fuse_small_kernel(Args a, long nbins) {
-    PIC_STATIC_SMEM(double, smem, SMALL_WARPS * group_bytes(SMALL_CAP) / 8);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    char* mine = reinterpret_cast<char*>(smem) + warp * group_bytes(SMALL_CAP);
-    const long stride = (long)gridDim.x * SMALL_WARPS;
-    for (long bin = (long)blockIdx.x * SMALL_WARPS + warp; bin < nbins; bin += stride) {
-        long cs1, cs2; int n1, n2;
-        const int n = cell_load(a, bin, &cs1, &n1, &cs2, &n2);
-        if (n == 0 || n > SMALL_CAP) continue;
-        fuse_cell<32>(a, bin, lane, mine, SMALL_CAP, cs1, n1, cs2, n2);
-    }
-}
-
-__global__ void __launch_bounds__(LARGE_THREADS) fuse_large_kernel(Args a, long nbins) {
-    PIC_DYNAMIC_SMEM(double, smem);
-    PIC_STATIC_SMEM(int, list, LARGE_SCAN + 1);
-    PIC_STATIC_SMEM(int, cnt, 4);
-    const int t = threadIdx.x;
-    for (long base = (long)blockIdx.x * LARGE_SCAN; base < nbins; base += (long)gridDim.x * LARGE_SCAN) {
-        if (t == 0) list[LARGE_SCAN] = 0;
-        __syncthreads();
-        const long bin = base + t;
-        if (t < LARGE_SCAN && bin < nbins) {
-            long cs1, cs2; int n1, n2;
-            if (cell_load(a, bin, &cs1, &n1, &cs2, &n2) > SMALL_CAP) list[atomicAdd(&list[LARGE_SCAN], 1)] = t;   // shared memory only
-        }
-        __syncthreads();
-        const int nl = list[LARGE_SCAN];
-        for (int k = 0; k < nl; ++k) {
-            const long b = base + list[k];
-            long cs1, cs2; int n1, n2;
-            const int n = cell_load(a, b, &cs1, &n1, &cs2, &n2);
-            if (n <= LARGE_CAP) fuse_cell<LARGE_THREADS>(a, b, t, reinterpret_cast<char*>(smem), LARGE_CAP, cs1, n1, cs2, n2);
-            else if (a.scr1 && (a.same || a.scr2)) fuse_cell_global(a, b, t, cnt, cs1, n1, cs2, n2);
-            else if (t == 0) *a.status = 1;
-        }
-        __syncthreads();
-    }
-}
 
 struct CreateArgs {
     SoaView P1, P2, PA, PB;
@@ -679,23 +455,13 @@ extern "C" long pic_fusion_workspace_bytes(long pair_capacity, long nbins) {
     return (long)total;
 }
 
-static int check_fusion(const char* what, const pic_fusion_collision* c, const pic_soa* p1, const pic_bins* b1,
-                        const pic_soa* p2, const pic_bins* b2) {
-    PIC_REQUIRE(c && p1 && b1, "%s: null argument", what);
-    PIC_REQUIRE(b1->cell_start && b1->np_binned == p1->np, "%s: species 1 needs current bins", what);
-    PIC_REQUIRE(p1->idcpu && p1->w, "%s: species 1 needs ids and weights", what);
+// the refusals about the reaction that both passes make
+static int check_fusion(const char* what, const pic_fusion_collision* c) {
     PIC_REQUIRE(c->type == PIC_FUSION_DT_NHE4 || c->type == PIC_FUSION_DD_PT || c->type == PIC_FUSION_DD_NHE3 ||
                 c->type == PIC_FUSION_PB_3HE4, "%s: unknown fusion type %d", what, c->type);
     PIC_REQUIRE(c->m1 > 0.0 && (c->same_species || c->m2 > 0.0) && c->mA > 0.0 &&
                 (c->type == PIC_FUSION_PB_3HE4 || c->mB > 0.0), "%s: masses must be positive", what);
     PIC_REQUIRE(c->fusion_multiplier > 0.0, "%s: the fusion multiplier must be positive", what);
-    if (!c->same_species) {
-        PIC_REQUIRE(p2 && b2 && b2->cell_start && b2->np_binned == p2->np && p2->idcpu && p2->w,
-                    "%s: species 2 needs current bins, ids and weights", what);
-        for (int d = 0; d < 3; ++d)
-            PIC_REQUIRE(b1->box_lo[d] == b2->box_lo[d] && b1->box_hi[d] == b2->box_hi[d] && b1->tile[d] == b2->tile[d],
-                        "%s: the two species' bins must describe the same box and tiles", what);
-    }
     return 0;
 }
 
@@ -703,47 +469,23 @@ extern "C" int pic_collide_nuclear_fusion(const pic_fusion_collision* c, const p
                                           const int* src1, const pic_soa* p2, const pic_bins* b2, const int* src2,
                                           const pic_geom* g, double dt, long step, int* scratch1, int* scratch2,
                                           void* work, long pair_capacity, int* status, void* stream) {
-    if (int rc = check_fusion("pic_collide_nuclear_fusion", c, p1, b1, p2, b2)) return rc;
-    PIC_REQUIRE(g && status && work, "pic_collide_nuclear_fusion: null argument");
-    PIC_REQUIRE(step >= 0, "pic_collide_nuclear_fusion: negative step");
+    const char* what = "pic_collide_nuclear_fusion";
+    fus::NuclearFusion::Args a;
+    if (int rc = coll::pair_args(what, c, p1, b1, src1, p2, b2, src2, g, dt, step, scratch1, scratch2, status, a))
+        return rc;
+    if (int rc = check_fusion(what, c)) return rc;
+    PIC_REQUIRE(work, "%s: null argument", what);
     const long need = c->same_species ? p1->np : p1->np + p2->np;
-    PIC_REQUIRE(pair_capacity >= need, "pic_collide_nuclear_fusion: the workspace holds %ld pairs, the reactants %ld",
-                pair_capacity, need);
-    fus::Args a;
-    a.P1 = make_soa(*p1, 0); a.id1 = p1->idcpu; a.src1 = src1; a.b1 = make_bins(*b1);
-    if (c->same_species) { a.P2 = a.P1; a.id2 = a.id1; a.src2 = a.src1; a.b2 = a.b1; }
-    else { a.P2 = make_soa(*p2, 0); a.id2 = p2->idcpu; a.src2 = src2; a.b2 = make_bins(*b2); }
-    a.gn[0] = g->n_cell[0]; a.gn[1] = g->n_cell[1];
-    double dx[3];
-    for (int d = 0; d < 3; ++d) dx[d] = (g->prob_hi[d] - g->prob_lo[d]) / g->n_cell[d];
-    a.dV = dx[0] * dx[1] * dx[2];
-    a.m1 = c->m1; a.m2 = c->m2; a.dt = dt;
+    PIC_REQUIRE(pair_capacity >= need, "%s: the workspace holds %ld pairs, the reactants %ld", what, pair_capacity, need);
     a.mult = c->fusion_multiplier; a.thr = c->fusion_probability_threshold; a.target = c->fusion_probability_target_value;
     a.type = c->type;
-    a.seed = c->seed; a.cidx = (uint64_t)(uint32_t)c->collision_index; a.step = (uint64_t)step; a.same = c->same_species;
-    a.scr1 = scratch1; a.scr2 = c->same_species ? nullptr : scratch2;
-    a.status = status;
     const long nbins = bins_count(a.b1);
     a.wk = fus::carve(work, pair_capacity, nbins);
     cudaStream_t s = (cudaStream_t)stream;
     cudaMemsetAsync(a.wk.npairs, 0, sizeof(int) * (size_t)(nbins + 1), s);
     cudaMemsetAsync(a.wk.events, 0, sizeof(int) * (size_t)(nbins + 1), s);
     if (p1->np == 0 || (!c->same_species && p2->np == 0)) return 0;
-    const long small_blocks = (nbins + fus::SMALL_WARPS - 1) / fus::SMALL_WARPS;
-    fus::fuse_small_kernel<<<(unsigned)(small_blocks < 2147483647L ? small_blocks : 2147483647L), fus::SMALL_WARPS * 32,
-                             0, s>>>(a, nbins);
-    count_launch();
-    static const size_t large_smem = fus::group_bytes(fus::LARGE_CAP);
-    static bool attr = [] {
-        return cudaFuncSetAttribute(fus::fuse_large_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)large_smem) == cudaSuccess;
-    }();
-    PIC_REQUIRE(attr, "pic_collide_nuclear_fusion: cannot reserve %zu bytes of shared memory", large_smem);
-    const long large_rounds = (nbins + fus::LARGE_SCAN - 1) / fus::LARGE_SCAN;
-    const long large_blocks = large_rounds < 16L * NUM_SMS ? large_rounds : 16L * NUM_SMS;
-    fus::fuse_large_kernel<<<(unsigned)large_blocks, fus::LARGE_THREADS, large_smem, s>>>(a, nbins);
-    count_launch();
-    return check_launch("pic_collide_nuclear_fusion") ? 0 : 1;
+    return coll::launch<fus::NuclearFusion>(what, a, s);
 }
 
 extern "C" int pic_fusion_create_products(const pic_fusion_collision* c, const pic_soa* p1, const pic_bins* b1,
@@ -751,7 +493,9 @@ extern "C" int pic_fusion_create_products(const pic_fusion_collision* c, const p
                                           void* work, long pair_capacity, const pic_soa* pA, long capA,
                                           uint64_t next_idA, const pic_soa* pB, long capB, uint64_t next_idB,
                                           long* n_events, void* stream) {
-    if (int rc = check_fusion("pic_fusion_create_products", c, p1, b1, p2, b2)) return rc;
+    PIC_REQUIRE(c && p1 && b1, "pic_fusion_create_products: null argument");
+    if (int rc = coll::check_species("pic_fusion_create_products", c->same_species, p1, b1, p2, b2)) return rc;
+    if (int rc = check_fusion("pic_fusion_create_products", c)) return rc;
     const bool pb = c->type == PIC_FUSION_PB_3HE4;
     PIC_REQUIRE(g && work && pA && (pb || pB) && n_events, "pic_fusion_create_products: null argument");
     PIC_REQUIRE(pA->idcpu && pA->w && (pb || (pB->idcpu && pB->w)),
