@@ -777,11 +777,63 @@ int pic_particles_mark_spent(const pic_soa* p, int* work, int cap, void* stream)
  * to a reactant or to the other product, ndt < 1, a bad type or parameter, fluid species, several ranks. */
 int pic_engine_add_fusion(void* engine, int isp1, int isp2, int iprodA, int iprodB, int type, double multiplier,
                           double probability_threshold, double probability_target_value, int ndt, uint64_t seed);
-/* The id counter of species isp: the id the next particle it creates receives (fusion products; ids next_id, next_id
- * + 1, ...).  It starts at the species' initial particle count; a checkpoint carries it.  The setter refuses a value
- * below the species' current count. */
+/* The id counter of species isp: the id the next particle it creates receives (fusion products, flux injection; ids
+ * next_id, next_id + 1, ...).  It starts at the species' initial particle count -- over several ranks the sum of the
+ * ranks' counts, which makes pic_engine_add_species a collective call there; a checkpoint carries it.  The setter
+ * refuses a value below the species' current count. */
 uint64_t pic_engine_species_next_id(void* engine, int isp);
 int pic_engine_set_species_next_id(void* engine, int isp, uint64_t next_id);
+
+/* ------------------------------------------------------------------------------------------
+ * Flux injection through a plane (<species>.injection_style = NFluxPerCell), 3D Cartesian, lab frame, a constant
+ * flux and momentum_distribution_type = gaussianflux: PlasmaInjector::setupNFluxPerCell
+ * (Source/Initialization/PlasmaInjector.cpp:295-385) and PhysicalParticleContainer::AddPlasmaFlux
+ * (Source/Particles/PhysicalParticleContainer.cpp:1336-1810); csrc/flux_injection.cu states the random streams and ids.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct pic_flux_injector {
+    double num_ppc;              /* <species>.num_particles_per_cell (real, > 0)                                   */
+    double surface_flux_pos;     /* <species>.surface_flux_pos [m]                                                 */
+    int normal_axis;             /* <species>.flux_normal_axis: 0 = x, 1 = y, 2 = z                                */
+    int direction;               /* <species>.flux_direction: +1 or -1                                             */
+    double flux;                 /* <species>.flux [m^-2 s^-1] (flux_profile = constant); <= 0 injects nothing     */
+    double tmin, tmax;           /* <species>.flux_tmin / flux_tmax [s]; < 0: unset                                */
+    double bound_lo[3], bound_hi[3];   /* xmin,ymin,zmin / xmax,ymax,zmax (+-inf when unset)                      */
+    double u_m[3], u_th[3];      /* ux_m.. / ux_th.. in units of c (InjectorMomentumGaussianFlux)                  */
+    uint64_t seed;               /* key of the Philox4x64-10 streams                                               */
+} pic_flux_injector;
+
+/* Device workspace of pic_add_flux_particles for injector inj on the domain g (any box of it); -1 and an error for an
+ * injector the library refuses (normal axis, direction, num_ppc, u_th, more than 2^31 particles per call). */
+long pic_flux_workspace_bytes(const pic_flux_injector* inj, const pic_geom* g);
+
+/* One step of PhysicalParticleContainer::ContinuousFluxInjection (PhysicalParticleContainer.cpp:2531-2540) ->
+ * AddPlasmaFlux (:1336-1810) for the box [box_lo, box_hi] of the domain g, at t = t_new (after cur_time += dt):
+ * nothing outside (tmin < 0 || t >= tmin) && (tmax < 0 || t < tmax).  The box owns the plane when box_lo <= pos < box_hi
+ * along the normal for direction > 0, box_lo < pos <= box_hi for direction < 0 (find_overlap_flux,
+ * AddPlasmaUtilities.cpp:45-109); each of its plane cells that overlaps the bounds draws int(num_ppc + Random)
+ * particles, at surface_flux_pos along the normal and uniform over the cell across it (InjectorPositionRandomPlane,
+ * InjectorPosition.H:33-63), with the Gaussian-flux normal momentum (SampleGaussianFluxDistribution.H, its sign flipped
+ * for direction < 0) and normal transverse momenta (InjectorMomentum.H:98-156), weight flux dx dy dz / num_ppc /
+ * dx[normal] dt (AddPlasmaUtilities.H:214-234), each then moved over t_fract = Random dt (UpdatePosition).  Particles
+ * outside the box or the bounds (inclusive) are dropped.  They are appended after p->np (the caller adds the return
+ * value to its count); ids first_id + cell (floor(num_ppc) + 1) + p for particle p of global plane cell cell, and
+ * *ids_used receives the ids the call used up on every box (0 outside the window).  step and injector_index are part
+ * of every random stream's counter.  work: pic_flux_workspace_bytes(inj, g) bytes (4 bytes per particle slot of the
+ * plane).  The particles are appended in slot order (cell-major, then p) without the dropped ones.  ONE host read of
+ * the count (synchronises `stream`); when p->np + the count would exceed capacity nothing is written and the call
+ * fails.  Returns the number appended, -1 on error. */
+long pic_add_flux_particles(const pic_flux_injector* inj, int injector_index, const pic_geom* g, const int box_lo[3],
+                            const int box_hi[3], long step, double t, double dt, const pic_soa* p, long capacity,
+                            uint64_t first_id, uint64_t* ids_used, void* work, long work_bytes, void* stream);
+
+/* One <species>.injection_style = NFluxPerCell source of species isp for the step driver: every step injects first in
+ * HandleParticlesAtBoundaries (Source/Evolve/WarpXEvolve.cpp:535), in the `flux_injection` stage, before the periodic
+ * wrap, the particle boundaries, the removal of spent reactants and the migration, which treat the injected particles
+ * like pushed ones; on bricks the brick that owns the plane cell creates them.  The species' id counter advances by
+ * the plane's cells times (floor(num_ppc) + 1) every injecting step.  The injector's index (the order of the calls)
+ * is part of its streams' counter.  Refused before the engine changes: a bad index or injector, a moving window, a
+ * boosted frame (pic_engine_set_boost refuses an engine with flux injectors). */
+int pic_engine_add_flux_injector(void* engine, int isp, const pic_flux_injector* inj);
 
 /* <species>.do_not_push / <species>.do_not_deposit of species isp for the step driver (0 or 1 each; both 0 is the
  * default).  do_not_push replaces the early returns of WarpXParticleContainer::PushX (WarpXParticleContainer.cpp:1478)

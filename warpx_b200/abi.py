@@ -90,6 +90,13 @@ class pic_fusion_collision(C.Structure):
                 ("seed", C.c_uint64), ("collision_index", C.c_int), ("same_species", C.c_int)]
 
 
+class pic_flux_injector(C.Structure):
+    _fields_ = [("num_ppc", C.c_double), ("surface_flux_pos", C.c_double), ("normal_axis", C.c_int),
+                ("direction", C.c_int), ("flux", C.c_double), ("tmin", C.c_double), ("tmax", C.c_double),
+                ("bound_lo", C.c_double * 3), ("bound_hi", C.c_double * 3), ("u_m", C.c_double * 3),
+                ("u_th", C.c_double * 3), ("seed", C.c_uint64)]
+
+
 FUSION_DT_NHE4, FUSION_DD_PT, FUSION_DD_NHE3, FUSION_PB_3HE4 = 0, 1, 2, 3
 SPENT_ID = 0xFFFFFFFFFFFFFFFF          # PIC_SPENT_ID: a reactant whose weight a fusion used up
 
@@ -141,6 +148,28 @@ def make_injector(ppc, bound_lo, bound_hi, density, do_continuous_injection=Fals
 
 
 DBL_MAX = 1.7976931348623157e308
+
+_AXES = {"x": 0, "y": 1, "z": 2}
+
+
+def make_flux_injector(num_particles_per_cell, surface_flux_pos, flux_normal_axis, flux_direction, flux=1.0,
+                       u_m=(0.0, 0.0, 0.0), u_th=(0.0, 0.0, 0.0), bound_lo=(-np.inf,) * 3, bound_hi=(np.inf,) * 3,
+                       flux_tmin=-1.0, flux_tmax=-1.0, seed=0):
+    """<species>.injection_style = NFluxPerCell by the deck's names: num_particles_per_cell (real), surface_flux_pos,
+    flux_normal_axis ("x", "y", "z" or 0..2), flux_direction (+1 / -1), flux (flux_profile = constant, or a
+    parse_flux_function that is a constant), u_m = (ux_m, uy_m, uz_m) and u_th = (ux_th, uy_th, uz_th) in units of c
+    (momentum_distribution_type = gaussianflux), bound_lo/hi = xmin..zmax, flux_tmin / flux_tmax (< 0: unset); seed
+    keys the injector's random streams."""
+    f = pic_flux_injector()
+    f.num_ppc, f.surface_flux_pos = float(num_particles_per_cell), float(surface_flux_pos)
+    f.normal_axis = _AXES[flux_normal_axis.lower()] if isinstance(flux_normal_axis, str) else int(flux_normal_axis)
+    f.direction, f.flux = int(flux_direction), float(flux)
+    f.tmin, f.tmax = float(flux_tmin), float(flux_tmax)
+    for d in range(3):
+        f.bound_lo[d], f.bound_hi[d] = float(bound_lo[d]), float(bound_hi[d])
+        f.u_m[d], f.u_th[d] = float(u_m[d]), float(u_th[d])
+    f.seed = int(seed)
+    return f
 
 
 def make_gaussian_beam(x_m, rms, npart, q_tot, u_m=(0.0, 0.0, 0.0), u_th=(0.0, 0.0, 0.0), cut=(DBL_MAX,) * 3,
@@ -209,6 +238,17 @@ def COLLISION_SIGNATURES(soap, bp, gp, vp):
         "pic_engine_set_species_flags": (C.c_int, [vp, C.c_int, C.c_int, C.c_int]),
         "pic_engine_add_fusion": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double,
                                             C.c_double, C.c_int, C.c_uint64]),
+    }
+
+
+def FLUX_SIGNATURES(soap, gp, ip, vp):
+    """ctypes signatures of the flux-injection entry points of include/pic_b200.h."""
+    fp = C.POINTER(pic_flux_injector)
+    return {
+        "pic_flux_workspace_bytes": (C.c_long, [fp, gp]),
+        "pic_add_flux_particles": (C.c_long, [fp, C.c_int, gp, ip, ip, C.c_long, C.c_double, C.c_double, soap, C.c_long,
+                                              C.c_uint64, C.POINTER(C.c_uint64), vp, C.c_long, vp]),
+        "pic_engine_add_flux_injector": (C.c_int, [vp, C.c_int, fp]),
     }
 
 

@@ -12,9 +12,10 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
          "-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
-# The fluid, collision and fusion kernels restate the reference's arithmetic operation by operation: no multiply-add
-# contraction there.
-FILE_FLAGS = {"fluid.cu": ["-fmad=false"], "collision.cu": ["-fmad=false"], "fusion.cu": ["-fmad=false"]}
+# The fluid, collision, fusion and flux-injection kernels restate the reference's arithmetic operation by operation: no
+# multiply-add contraction there.
+FILE_FLAGS = {"fluid.cu": ["-fmad=false"], "collision.cu": ["-fmad=false"], "fusion.cu": ["-fmad=false"],
+              "flux_injection.cu": ["-fmad=false"]}
 
 
 def sources():

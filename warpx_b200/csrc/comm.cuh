@@ -11,7 +11,7 @@ namespace pic {
 struct PicNcclUniqueId { char internal[128]; };
 typedef struct ncclComm* PicNcclComm;
 constexpr int PIC_NCCL_INT32 = 2, PIC_NCCL_FLOAT64 = 8;   // ncclDataType_t
-constexpr int PIC_NCCL_MAX = 2;                           // ncclRedOp_t
+constexpr int PIC_NCCL_SUM = 0, PIC_NCCL_MAX = 2;          // ncclRedOp_t
 
 struct NcclApi {
     bool loaded = false;

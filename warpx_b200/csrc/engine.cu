@@ -33,6 +33,7 @@
 namespace pic {
 
 bool gather_push_carries_permutation(int nox);      // gather_push.cu
+int flux_list_escapes(const pic_escape_list* e, long first, long n, void* stream);   // flux_injection.cu
 
 // Memory the engine owns: device memory, or pinned host memory when Pinned.  The only code in this file that
 // allocates or frees; the memory goes with its owner.  Empty (null) until an allocation succeeds.
@@ -104,6 +105,13 @@ private:
     bool has_bins_ = false, exact_ = false, stale_ = false, esc_valid_ = false;
 };
 
+// One <species>.injection_style = NFluxPerCell source (pic_engine_add_flux_injector) with its workspace
+struct FluxInjector {
+    pic_flux_injector prm;
+    int index;                   // position among the engine's flux injectors: part of its streams' counter
+    DeviceBuf<char> work;
+};
+
 struct Species {
     Species(double q_, double m_, const pic_bins& bins) : q(q_), m(m_), ord(bins) {}
     double q, m;
@@ -136,6 +144,7 @@ struct Species {
     int spent_cap = 0;
     bool do_not_push = false;      // <species>.do_not_push: x and u keep their bits (pic_engine_set_species_flags)
     bool do_not_deposit = false;   // <species>.do_not_deposit: no current deposition
+    std::vector<FluxInjector> flux;
 };
 
 // Laser antenna: its own particle container (LaserParticleContainer), no gather, order-agnostic deposit
@@ -152,10 +161,10 @@ struct Laser {
 // recorded on the stream the stages are launched on, inside the same pic_engine_evolve calls a benchmark times.
 enum { ST_FILL_EB = 0, ST_GATHER_PUSH, ST_ZERO_J, ST_DEPOSIT, ST_SYNC_J, ST_EVOLVE_B, ST_FILL_B, ST_EVOLVE_E, ST_FILL_E,
        ST_WRAP, ST_MIGRATE, ST_SORT, ST_NCI, ST_WINDOW, ST_PUSHP, ST_FILTER, ST_FLUID_GATHER_PUSH, ST_FLUID_FILL,
-       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COLLISIONS, ST_FUSION, ST_FUSION_PRODUCTS, ST_COUNT };
+       ST_FLUID_ADVECT, ST_FLUID_DEPOSIT, ST_COLLISIONS, ST_FUSION, ST_FUSION_PRODUCTS, ST_FLUX_INJECTION, ST_COUNT };
 static const char* const stage_names[ST_COUNT] = {"fill_boundary_eb", "gather_push", "zero_j", "deposit", "sync_current",
     "evolve_b", "fill_boundary_b", "evolve_e", "fill_boundary_e", "wrap", "migrate", "sort", "nci_filter", "move_window", "push_p", "filter_j",
-    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit", "collisions", "fusion", "fusion_products"};
+    "fluid_gather_push", "fluid_fill_boundary", "fluid_advect", "fluid_deposit", "collisions", "fusion", "fusion_products", "flux_injection"};
 // Cold fluid species (WarpXFluidContainer): two borrowed states of N, NUx, NUy, NUz; the advection writes one from the
 // other and `cur` names the current one.
 struct Fluid {
@@ -232,6 +241,7 @@ struct Engine {
     std::vector<Fluid> fluids;
     std::vector<Collision> collisions;
     DeviceBuf<int> coll_status;                  // a cell exceeded the collision kernel's capacity
+    int n_flux = 0;                              // flux injectors of all species
 };
 
 struct Stage {      // records the events of one stage when timing is on
@@ -869,6 +879,31 @@ static int remove_spent(Engine& e, void* stream) {
     }, "spent-reactant pass", s);
 }
 
+// PhysicalParticleContainer::ContinuousFluxInjection (PhysicalParticleContainer.cpp:2531-2540), the first thing
+// HandleParticlesAtBoundaries does (WarpXEvolve.cpp:535): each injector's particles of this step go behind the species'
+// particles and join its escape list, so that the wrap, the particle boundaries and the migration of the step treat
+// them as pushed particles.
+static int flux_injection(Engine& e, long step, void* s) {
+    for (auto& sp : e.species) {
+        if (sp.flux.empty()) continue;
+        ENG_CALL(apply_pending(sp, s));
+        pic_soa& P = sp.buf[sp.cur];
+        const long np0 = P.np;
+        for (auto& f : sp.flux) {
+            uint64_t used = 0;
+            const long n = pic_add_flux_particles(&f.prm, f.index, &e.geom, e.box_lo, e.box_hi, step, e.cur_time, e.dt, &P,
+                                                  sp.capacity, sp.next_id, &used, f.work.get(), (long)f.work.bytes(), s);
+            if (n < 0) return 1;
+            P.np += n;
+            sp.next_id += used;
+        }
+        if (P.np == np0) continue;
+        sp.ord.cells_changed();
+        if (sp.has_esc()) ENG_CALL(flux_list_escapes(&sp.esc, np0, P.np - np0, s));
+    }
+    return 0;
+}
+
 // last: Synchronize() ends the step; defer_sort: another step of the same call follows, its push moves the sorted particles
 static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     // ---- ExplicitFillBoundaryEBUpdateAux ----
@@ -911,6 +946,7 @@ static int one_step(Engine& e, bool last, bool defer_sort, void* s) {
     int num_moved = 0;
     { Stage t(e, ST_WINDOW, s); ENG_CALL(move_window(e, e.is_synchronized, &num_moved, s)); }
     // ---- HandleParticlesAtBoundaries ----
+    if (e.n_flux) { Stage t(e, ST_FLUX_INJECTION, s); ENG_CALL(flux_injection(e, step, s)); }
     {
         Stage t(e, ST_WRAP, s);
         for (auto& sp : e.species) {
@@ -1033,6 +1069,22 @@ extern "C" int pic_engine_set_fields(void* h, const pic_fab fabs[9]) {
                     d, e->box_hi[d] - e->box_lo[d] + 1, e->ng_J[d]);
     return 0;
 }
+// Over several ranks (collective): the sum of n over the ranks, the particle count of the single box that would hold
+// every brick's particles.  A new species' id counter starts there on every rank, so that the ids a species creates
+// later (flux injection) are the same on any decomposition.
+static int global_count(Engine& e, long n, uint64_t* out, void* stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    DeviceBuf<double> d;
+    ENG_CALL(d.alloc(sizeof(double), "pic_engine_add_species: cannot allocate the count scratch"));
+    double v = (double)n;            // exact below 2^53
+    cudaMemcpyAsync(d.get(), &v, sizeof(double), cudaMemcpyHostToDevice, s);
+    ENG_NCCL(g_nccl.AllReduce(d.get(), d.get(), 1, PIC_NCCL_FLOAT64, PIC_NCCL_SUM, e.comm->comm, s));
+    cudaMemcpyAsync(&v, d.get(), sizeof(double), cudaMemcpyDeviceToHost, s);
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail("pic_engine_add_species: %s", cudaGetErrorString(cudaGetLastError()));
+    *out = (uint64_t)v;
+    return 0;
+}
+
 // bufA holds the particles; bufB is the sort target.  cell_start / sort_work may be NULL (no bins).
 extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa* bufA, const pic_soa* bufB,
                                       long capacity, int* cell_start, const int tile[3], void* sort_work,
@@ -1080,6 +1132,7 @@ extern "C" int pic_engine_add_species(void* h, double q, double m, const pic_soa
         cudaMemsetAsync(sp.mig_work.get(), 0, (size_t)pic_migrate_workspace_bytes(sp.mig_cap_max), (cudaStream_t)stream);
     }
     if (!e->all_periodic) ENG_CALL(alloc_boundary_scratch(capacity, sp.bnd_work, &sp.bnd_cap));
+    if (e->comm) ENG_CALL(global_count(*e, (long)bufA->np, &sp.next_id, stream));
     PinnedBuf<int> counts;
     ENG_CALL(alloc_host_counts_for_one_more(*e, counts));
     if (cell_start && sort_work) ENG_CALL(sort_species(*e, sp, false, stream));
@@ -1202,6 +1255,7 @@ extern "C" int pic_engine_set_boost(void* h, double gamma_boost, double beta_boo
     PIC_REQUIRE((gamma_boost > 1.) == (beta_boost > 0.), "pic_engine_set_boost: gamma_boost and beta_boost disagree");
     PIC_REQUIRE(e->lasers.empty(), "pic_engine_set_boost: call before pic_engine_add_laser");
     for (auto& sp : e->species) PIC_REQUIRE(!sp.has_injector, "pic_engine_set_boost: call before pic_engine_set_injector");
+    PIC_REQUIRE(e->n_flux == 0, "pic_engine_set_boost: boosted frames take no flux injection");
     e->gamma_boost = gamma_boost; e->beta_boost = beta_boost;
     return 0;
 }
@@ -1419,6 +1473,24 @@ extern "C" int pic_engine_set_species_next_id(void* h, int isp, uint64_t next_id
     PIC_REQUIRE(next_id >= (uint64_t)sp.buf[sp.cur].np, "pic_engine_set_species_next_id: %llu is below the %ld particles",
                 (unsigned long long)next_id, (long)sp.buf[sp.cur].np);
     sp.next_id = next_id;
+    return 0;
+}
+
+// One NFluxPerCell source of species isp (include/pic_b200.h); refused before the engine changes.
+extern "C" int pic_engine_add_flux_injector(void* h, int isp, const pic_flux_injector* inj) {
+    Engine* e = static_cast<Engine*>(h);
+    PIC_REQUIRE(e && inj, "pic_engine_add_flux_injector: null argument");
+    PIC_REQUIRE(isp >= 0 && isp < (int)e->species.size(), "pic_engine_add_flux_injector: no species %d", isp);
+    PIC_REQUIRE(!e->do_moving_window, "pic_engine_add_flux_injector: runs with a moving window take no flux injection");
+    PIC_REQUIRE(!(e->gamma_boost > 1.0), "pic_engine_add_flux_injector: boosted frames take no flux injection");
+    const long bytes = pic_flux_workspace_bytes(inj, &e->geom);
+    if (bytes < 0) return 1;
+    FluxInjector f;
+    f.prm = *inj;
+    f.index = e->n_flux;
+    ENG_CALL(f.work.alloc((size_t)bytes, "pic_engine_add_flux_injector: cannot allocate the injection workspace"));
+    e->species[isp].flux.push_back(std::move(f));
+    ++e->n_flux;
     return 0;
 }
 

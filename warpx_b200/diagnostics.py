@@ -248,8 +248,9 @@ def write_checkpoint(sim, prefix, iteration=None, file_min_digits=5):
         if rank == 0:
             ntot = int(sum(c[0] for c in counts))
             # the next-id field, 1-based as AMReX's ids: the species' id counter + 1 (at least ntot + 1); fusion products
-            # continue from it after a restart
-            next_id = max(ntot, sim.species_next_id(isp)) + 1 if sim.world == 1 else ntot + 1
+            # and injected particles continue from it after a restart.  Over several ranks the counter is the same on
+            # every rank (it starts at the global count and advances by global amounts).
+            next_id = max(ntot, sim.species_next_id(isp)) + 1
             with open(os.path.join(root, sp.name, "Header"), "w") as f:
                 f.write("Version_Two_Dot_Zero_double\n3\n4\nw\nux\nuy\nuz\n0\n1\n%d\n%d\n0\n%d\n" % (ntot, next_id, world))
                 for r in range(world):
@@ -302,7 +303,7 @@ def read_checkpoint(sim, root, capacity=None):
         sim.add_species(name, float(q), float(m), *[np.ascontiguousarray(rec[:, k]) for k in range(7)], ids=ids,
                         species_type=stype[0] if stype else None,
                         capacity=(capacity or {}).get(name))
-        if sim.world == 1 and int(ph[10]) - 1 > count:
+        if int(ph[10]) - 1 > count:
             sim.set_species_next_id(isp, int(ph[10]) - 1)
     sim.set_step(istep, time)
     sim.is_synchronized = True

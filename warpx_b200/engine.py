@@ -333,6 +333,7 @@ class Simulation:
         if not self.native:
             raise RuntimeError("pic_b200: " + self.L.pic_last_error().decode())
         self.collisions = []
+        self.flux_injectors = []
         if boundaries is not None:
             check(self.L.pic_engine_set_boundaries(self.native, C.byref(boundaries)))
         if moving_window is not None:
@@ -576,6 +577,24 @@ class Simulation:
                                     probability_target_value=float(probability_target_value), ndt=int(ndt),
                                     seed=int(seed)))
         return len(self.collisions) - 1
+
+    def add_flux_injection(self, species, injector):
+        """A source of particles through a plane for species (a Species object, name or index): injector is an
+        abi.pic_flux_injector from abi.make_flux_injector and stands for <species>.injection_style = NFluxPerCell with
+        <species>.num_particles_per_cell, surface_flux_pos, flux_normal_axis, flux_direction, flux_tmin, flux_tmax,
+        xmin..zmax, flux_profile = constant with <species>.flux (or a constant parse_flux_function) and
+        momentum_distribution_type = gaussianflux with ux_m..uz_m, ux_th..uz_th.  Every step then injects
+        int(num_particles_per_cell + Random) particles per plane cell, weighted by flux dt, before the step's particle
+        boundaries and migration (PhysicalParticleContainer::AddPlasmaFlux).  The species needs the capacity for what
+        the run injects.  Lab frame only: runs with a moving window or a boosted frame are refused.  The injector's
+        index (the order of these calls) is part of its random streams; a restarted run registers its injectors
+        again, in the same order.  Returns the index."""
+        if self.moving_window is not None or self.gamma_boost > 1.0:
+            raise NotImplementedError("flux injection: lab-frame runs without a moving window only")
+        isp = self._species_index(species)
+        check(self.L.pic_engine_add_flux_injector(self.native, isp, C.byref(injector)))
+        self.flux_injectors.append((isp, injector))
+        return len(self.flux_injectors) - 1
 
     def set_species_flags(self, species, do_not_push=False, do_not_deposit=False):
         """<species>.do_not_push / <species>.do_not_deposit of a species (a Species object, name or index), also one that

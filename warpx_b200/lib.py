@@ -133,6 +133,7 @@ def bind(L):
     sig.update(abi.LWFA_SIGNATURES(fabp, soap, gp, bndp, lasp, injp, dp, ip, vp))
     sig.update(abi.FLUID_SIGNATURES(fabp, dp, vp))
     sig.update(abi.COLLISION_SIGNATURES(soap, bp, gp, vp))
+    sig.update(abi.FLUX_SIGNATURES(soap, gp, ip, vp))
     for name, (res, args) in sig.items():
         fn = getattr(L, name)      # AttributeError if include/pic_b200.h and the library disagree
         fn.restype = res

@@ -565,3 +565,31 @@ def proton_boron_3d(scale=1.0, seed=6):
                 analysis=dict(reaction="pb", E_step=E_step, sets=sets, tol=1e-12, energy_tol=1e-8, isotropy=0.03,
                               thermal_isotropy=0.1, xy_isotropy=0.05, thermal=dict(T_keV=44.0, n_p=1e28, n_b=5e28,
                                                                                     tolerance=0.2), rho_tol=2e-11))
+
+
+# ---- the reference's 3D flux-injection deck (Examples/Tests/flux_injection/inputs_test_3d_flux_injection) ------------
+M_P = 1.67262192369e-27
+
+
+def flux_injection_3d(n=16, ppc=100.0, max_step=2, seed=7):
+    """Examples/Tests/flux_injection/inputs_test_3d_flux_injection: n^3 cells over [-4, 4]^3 m, periodic,
+    algo.maxwell_solver = none with warpx.const_dt = 7e-9, shape order 3, max_step steps; four empty species fed through
+    planes (injection_style = NFluxPerCell, num_particles_per_cell = ppc, flux 1 m^-2 s^-1, gaussianflux momenta with
+    u_th = 0.1 on every axis): electrons through y = -4 towards +y with uy_m = 0.07, protons through x = +4 towards -x
+    with ux_m = 0.05, "negative" electrons through z = -4 towards +z with uz_m = -0.07, "negative" protons through
+    z = +4 towards -z with uz_m = -0.05.  Each species gets the capacity of max_step full injections.  The analysis
+    (analysis_flux_injection_3d.py) histograms the momenta of each species against N_tot = flux 64 m^2 t_max times a
+    Gaussian (transverse, within 0.07 of the peak) or a Gaussian-flux distribution (normal, within 0.05)."""
+    th = (0.1, 0.1, 0.1)
+    cap = int(max_step * n * n * (int(ppc) + 1))
+    sources = [("electron", -Q_E, M_E, "y", -4.0, +1, (0.0, 0.07, 0.0)),
+               ("proton", Q_E, M_P, "x", 4.0, -1, (0.05, 0.0, 0.0)),
+               ("electron_negative", -Q_E, M_E, "z", -4.0, +1, (0.0, 0.0, -0.07)),
+               ("proton_negative", Q_E, M_P, "z", 4.0, -1, (0.0, 0.0, -0.05))]
+    species = [dict(name=name, q=q, m=m, capacity=cap,
+                    flux=dict(num_particles_per_cell=ppc, surface_flux_pos=pos, flux_normal_axis=axis,
+                              flux_direction=direction, flux=1.0, u_m=u_m, u_th=th, seed=seed))
+               for name, q, m, axis, pos, direction, u_m in sources]
+    return dict(n_cell=(n, n, n), prob_lo=(-4.0, -4.0, -4.0), prob_hi=(4.0, 4.0, 4.0), nox=3, dt=7e-9, max_step=max_step,
+                species=species, analysis=dict(flux=1.0, emission_surface=8 * 8, hist_bins=50, hist_range=(-0.5, 0.5),
+                                               gaussian_tol=0.07, flux_tol=0.05))
